@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — GSO-update throughput on B200 (the BASELINE.json metric), one JSON line on stdout.
+"""bench.py — GSO-update throughput on H100 (the BASELINE.json metric), one JSON line on stdout.
 
 Step  = what LLLReduction::babai pays per iteration on the GSO state of every lattice of a batch
         (lll.cpp:166-224):  row_op_end(kappa, kappa+1)  [update_bf + Gram/GSO invalidation, gso_interface.cpp:32-53]
@@ -15,6 +15,10 @@ e2e   = same metric through the C-ABI with HOST buffers: every step uploads each
         reads rows kappa of mu and r back (b200gso_get_mu_r_row) — the protocol of a host-resident LLL driver.
 --impl reference : the UNMODIFIED reference (oracle/_ref/ref_probe over libfplll.so) doing the same step on the
         box's host cores, all threads; bounded sample.
+--dump-outputs DIR : after the timed steps, rows kappa of mu and r of every lattice as the device-resident path left
+        them (update_row_mu.npy, update_row_r.npy) and as the last end-to-end step read them back (e2e_mu.npy,
+        e2e_r.npy), float64; a fixed sample of lattices when the batch would pass 64 MB.  The inputs are seeded, so
+        two builds run with the same arguments can be compared array for array.
 """
 import argparse
 import json
@@ -37,21 +41,11 @@ def alg_bytes_update_row(i, n, g=1):
     return 8 * ((i + 1) * n * g + i * (i - 1) // 2 + 4 * (i + 1))
 
 
-def ncu_traffic(batch):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of k_update_row from the committed ncu capture, if it was
-    taken at this batch size (else None)."""
-    try:
-        j = json.load(open(os.path.join(ROOT, "profiles", "update_row_ncu_traffic.json")))
-        return j["dram_bytes_per_launch"] if int(j["batch"]) == int(batch) else None
-    except Exception:
-        return None
-
-
 def measure_traffic(batch, local):
     """dram__bytes_read.sum + dram__bytes_write.sum of ONE launch of k_update_row, measured now: `ncu --metrics ...` around
     a child of this script (`--traffic-child`) that builds the same state and launches the kernel a few times.  Hardware
     counters cannot be read from inside an unprofiled run, and nothing timed runs under the profiler.  None if ncu is not
-    usable on this box (the committed capture is reported instead)."""
+    usable on this box."""
     import csv
     import io
     try:
@@ -93,8 +87,8 @@ def traffic_child(batch):
 def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
-        return json.load(open(p)).get("hbm_gbs", 6650.0), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return json.load(open(p)).get("hbm_gbs", 3350.0), "measured (MEASURED_PEAKS.json hbm_gbs)"
+    return 3350.0, "H100 SXM data sheet HBM3 bandwidth (3.35 TB/s), not measured"
 
 
 class ClockSampler:
@@ -232,7 +226,7 @@ def hh_extras(local):
         from fplll_b200.householder import MatHouseholder
         d = n = 400
         i = d - 1
-        B = int(os.environ.get("B200_BENCH_HH_BATCH", 2960))  # 2960 = the resident warps of hk_update_R<14> on 148 SMs
+        B = int(os.environ.get("B200_BENCH_HH_BATCH", 2640))  # 20 resident warps of hk_update_R<14> x 132 SMs of an H100
         rng = np.random.default_rng(7)
         b = rng.integers(-(1 << 20), 1 << 20, size=(1, d, n), dtype=np.int64)
         m = MatHouseholder(np.broadcast_to(b, (B, d, n)), 5, device=local, keep_history=False)
@@ -271,7 +265,7 @@ def bkz_extras(local, devices=None, with_ref=True):
         # failed attempt is retried with the next rerandomisation seed, every attempt is reported
         # Every SVP call enumerates the fixed region of its initial radius (include/b200bkz.h: the default), so a tour is a
         # function of (basis, seed) alone: seeds 1 and 3 end with status 8, seed 2 in RED_BABAI_FAILURE near the end of the
-        # tour — every time, on any number of devices (profiles/r2_bkz60_runs.txt).
+        # tour — every time, on any number of devices.
         attempts = []
         for seed in (1, 3, 2):
             b = g["b"].copy()
@@ -313,10 +307,28 @@ def bkz_child(ndev):
     return 0
 
 
+DUMP_LIMIT = 64 << 20
+
+
+def dump_outputs(path, arrays, rank=0):
+    """arrays: name -> (batch, ...) float64.  Rank r > 0 writes <name>_rank<r>.npy.  Over DUMP_LIMIT bytes in all, the
+    same seeded sample of lattices is taken from every array."""
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    total = sum(v.nbytes for v in arrays.values())
+    batch = len(next(iter(arrays.values())))
+    keep = None
+    if total > DUMP_LIMIT:
+        keep = np.sort(np.random.default_rng(0).choice(batch, batch * DUMP_LIMIT // total, replace=False))
+    for name, v in arrays.items():
+        v = np.asarray(v, dtype=np.float64)
+        np.save(os.path.join(path, name + ("_rank%d" % rank if rank else "") + ".npy"), v if keep is None else v[keep])
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=200)  # 0.56 ms per step: ~0.1 s device-timed + ~0.25 s end to end
+    ap.add_argument("--steps", type=int, default=200)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--batch", type=int, default=0, help="lattices per GPU (0 = two full waves of the update kernel)")
@@ -326,6 +338,7 @@ def main():
     ap.add_argument("--bkz-child", type=int, default=0, help=argparse.SUPPRESS)
     ap.add_argument("--traffic-child", type=int, default=0, help=argparse.SUPPRESS)
     ap.add_argument("--no-traffic", action="store_true", help="skip the live ncu measurement of the kernel's DRAM traffic")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the timed steps computed as DIR/<name>.npy")
     a = ap.parse_args()
     if a.bkz_child:
         return bkz_child(a.bkz_child)
@@ -406,10 +419,15 @@ def main():
         dist.barrier()
     value = world * B * per_lat * a.steps / (ms_total * 1e-3) / 1e9
     kern_gbps = B * per_lat / (ms_update * 1e-3) / 1e9
+    dumps = {}
+    if a.dump_outputs:
+        mu, r, _ = m.get_mu_r_row(KAPPA)
+        dumps.update(update_row_mu=mu, update_row_r=r)
 
     # ---- end to end through the C-ABI with host buffers ---------------------------------------------------
     # host buffers are pinned (cudaHostAlloc via torch): the C-ABI takes plain host pointers, pinned ones DMA directly
-    rows = torch.randint(-(1 << 20), 1 << 20, (B, N_COLS), dtype=torch.int64).pin_memory().numpy()
+    rows = torch.randint(-(1 << 20), 1 << 20, (B, N_COLS), dtype=torch.int64,
+                         generator=torch.Generator().manual_seed(4321 + rank)).pin_memory().numpy()
     out = (torch.empty((B, D), dtype=torch.float64).pin_memory().numpy(),
            torch.empty((B, D), dtype=torch.float64).pin_memory().numpy(),
            torch.empty((B,), dtype=torch.int32).pin_memory().numpy())
@@ -429,6 +447,9 @@ def main():
     torch.cuda.synchronize()
     e2e_s = time.perf_counter() - t0
     assert (v == KAPPA + 1).all()  # every lattice's row kappa is valid through the diagonal
+    if a.dump_outputs:
+        dumps.update(e2e_mu=out[0].copy(), e2e_r=out[1].copy())
+        dump_outputs(a.dump_outputs, dumps, rank)
     if dist:
         t = torch.tensor([e2e_s], device="cuda", dtype=torch.float64)
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -495,16 +516,15 @@ def main():
         m.close()  # the child needs the memory
         m = None
         traffic = measure_traffic(B, local)
-        traffic_src = "measured in this run: ncu dram__bytes_read.sum + dram__bytes_write.sum of one k_update_row launch (child process)"
-    if traffic is None:
-        traffic, traffic_src = ncu_traffic(B), "profiles/update_row_ncu_traffic.json (committed ncu --set full capture)"
+        traffic_src = ("measured in this run: ncu dram__bytes_read.sum + dram__bytes_write.sum of one k_update_row launch "
+                       "(child process)" if traffic is not None else "not measured: ncu is not usable here")
     if rank == 0:
         peak, peak_src = peaks()
         line = {"metric": METRIC, "value": value, "unit": "GB/s", "n_gpus": world, "steps": a.steps,
                 "warmup": a.warmup, "ms_per_step": ms_total / a.steps, "higher_is_better": True, "scaling": "weak",
                 "vs_baseline": None, "dtype": "f64", "data": "synthetic",
                 "config": {"workload": workload_str(B), "batch": B, "entries": "uniform int in [-2^20, 2^20)", "flags": "GSO_ROW_EXPO",
-                           "state_bytes_per_gpu": int(B * 1.39e6), "l2": "inputs larger than L2 (state >> 126 MB)",
+                           "state_bytes_per_gpu": int(B * 1.39e6), "l2": "inputs larger than L2 (state >> 50 MB)",
                            "algorithmic_bytes_per_lattice": per_lat},
                 "roofline": {"bound": "hbm", "kernel": "k_update_row (update_gso_row, g=1)", "achieved": kern_gbps,
                              "peak": peak, "unit": "GB/s", "frac": kern_gbps / peak, "peak_source": peak_src,

@@ -1,9 +1,9 @@
-"""fplll_b200 — B200-native fp64 Gram-Schmidt / LLL inner loop and BKZ enumeration behind fplll's API.
+"""fplll_b200 — GPU-native (H100) fp64 Gram-Schmidt / LLL inner loop and BKZ enumeration behind fplll's API.
 
 Host-side mirror of the reference classes (same method names, argument meaning and error behaviour):
   MatGSO          <- fplll/gso.h:33 MatGSO<Z_NR<long>, FP_NR<double>>
   lll_reduction   <- fplll/wrapper.h:136 (the <long,double> stage)
-All compute happens in hand-written sm_100a kernels behind the C-ABI of include/*.h.
+All compute happens in hand-written sm_90a kernels behind the C-ABI of include/*.h.
 """
 from ._lib import B200Error  # noqa: F401
 from .gso import MatGSO, lll_reduction, GSO_DEFAULT, GSO_ROW_EXPO, GSO_OP_FORCE_LONG  # noqa: F401

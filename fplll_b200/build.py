@@ -1,4 +1,4 @@
-"""In-tree nvcc build of the CUDA extension (sm_100a only).  The .so stays in fplll_b200/lib/ (git-ignored,
+"""In-tree nvcc build of the CUDA extension (sm_90a, H100, only).  The .so stays in fplll_b200/lib/ (git-ignored,
 travels to the GPU box with the snapshot)."""
 import os
 import subprocess
@@ -7,7 +7,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 # B200_LIB_DIR: build/load a variant (other -D flags) next to the default one; the default is what ships
 LIBDIR = os.path.join(HERE, os.environ.get("B200_LIB_DIR", "lib"))
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = ARCH + [ "-lineinfo", "-O3", "-std=c++17",
               # the reference build never contracts a*b+c (configure.ac:25: -O3, no -march): bit parity needs the same
               "--fmad=false", "-Xcompiler", "-fPIC", "-shared"]
 
@@ -65,7 +66,7 @@ def build_all(force=False, verbose=False):
         out = os.path.join(LIBDIR, name)
         deps = [objs[u] for u in srcs]
         if force or not os.path.exists(out) or any(os.path.getmtime(o) > os.path.getmtime(out) for o in deps):
-            cmd = ["nvcc", "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", out] + deps
+            cmd = ["nvcc", "-shared"] + ARCH + ["-o", out] + deps
             if name == "libb200enum.so" and os.environ.get("B200_WITH_NCCL"):
                 cmd += ["-lnccl"]
             subprocess.check_call(cmd)

@@ -1,9 +1,9 @@
-// enum_api.cu — B200-native Schnorr-Euchner enumeration (BKZ's SVP subtree search) behind include/b200enum.h.
+// enum_api.cu — GPU-native Schnorr-Euchner enumeration (BKZ's SVP subtree search) behind include/b200enum.h.
 //
 // Reference algorithm: EnumerationBase::enumerate_loop (fplll/enum/enumerate_base.cpp:152-254) + next_pos_up
 // (enumerate_base.h:145-171); the only parallel strategy in the reference is enumlib's subtree fan-out over
 // std::threads with one shared radius and a shared subtree counter (fplll/enum-parallel/enumeration.h:62-81,
-// 382-510).  B200 design:
+// 382-510).  Device design:
 //   1. HOST BREADTH PHASE  — the top T levels (d-1 .. d-T) are expanded level by level, each level in exact
 //      Schnorr-Euchner order, into subtree roots (x[d-T..d-1], partial length).  T grows until there are enough roots
 //      to seed the machine.  Roots are sorted by partial length so the most promising subtrees run first (enumlib does
@@ -67,7 +67,7 @@ constexpr int THREADS_XS = 512;      // upper bound of the CTA size of the x-in-
 constexpr int MIN_ROOTS  = 128;      // host breadth phase: grow T until at least this many roots (the device multiplies
                                      // them by work splitting, a round costs one grid barrier) ...
 constexpr int MAX_ROOTS  = 1 << 15;  // ... but never beyond this (the pinned staging block is sized for it)
-constexpr int SMEM_XS_MAX = 227 * 1024;  // opt-in dynamic shared memory per CTA on sm_100
+constexpr int SMEM_XS_MAX = 227 * 1024;  // opt-in dynamic shared memory per CTA on sm_90
 constexpr unsigned TASK_CAP = 1u << 21;  // device task queue capacity (tasks of one round)
 constexpr int MAX_PEERS = 8;
 constexpr unsigned long long INF_BITS = 0x7ff0000000000000ull;
@@ -166,7 +166,7 @@ __device__ inline unsigned long long atomic_add_sys(unsigned long long *p, unsig
 // XS = true (dim <= 64, every BKZ block size in use; primal, no sub-solutions): the coefficient vectors x[] of all
 // walkers of the CTA live in SHARED memory ([level][thread], conflict-free) — the centre chain reads x[j] d-k times per
 // node, and with x[] in thread-local memory that traffic (L1 misses for 3/4 of it, ~1.6 KB of L2 reads per node) was
-// what bounded the first version (profiles/r1_enum_ncu.txt).  One CTA per SM then shares a single copy of mu^T.
+// what bounded the first version.  One CTA per SM then shares a single copy of mu^T.
 // Both variants also keep pre[k] = the part of level k's centre chain that only involves the task's FIXED coefficients
 // (j > top0): it is computed the first time the walker reaches level k inside a task and is the exact prefix of the
 // reference's descending chain, so the remaining chain is top0-k long instead of d-1-k.
@@ -703,15 +703,14 @@ const Tuning &tuning()
     q.use_xs         = (int)geti("B200_ENUM_XS", 1);
     q.xs_threads_cap = (int)geti("B200_ENUM_XS_THREADS", 320);
     // hand-off threshold: a call that has visited this many nodes on the first device and still has work pending is
-    // spread over all devices.  200 M nodes = ~25 ms of one B200.  With 32 M the BKZ-60 tour on two devices spent 7.0 s
-    // in enumeration against 4.5 s on one (fixed-region calls of 30-100 M nodes are common, and suspending at a round
-    // boundary + peer copies + a cooperative launch and a read-back per device cost more than half such a call saves):
-    // a tour must never pay for devices it cannot use.
+    // spread over all devices.  A low threshold makes a BKZ-60 tour on two devices slower than on one (fixed-region
+    // calls of 30-100 M nodes are common, and suspending at a round boundary + peer copies + a cooperative launch and a
+    // read-back per device cost more than half such a call saves): a tour must never pay for devices it cannot use.
     q.fan_nodes = (unsigned long long)geti("B200_ENUM_FAN_NODES", 200000000);
     q.min_roots   = (int)geti("B200_ENUM_MIN_ROOTS", MIN_ROOTS);
     q.shard_roots = (int)geti("B200_ENUM_SHARD_ROOTS", 8192);
-    // rounds with fewer tasks than warps are bound by the latency of a lone walker (~0.35 us per node): yield sooner
-    q.yield_small = (unsigned)geti("B200_ENUM_YIELD_SMALL", 8);  // BKZ-60 tour: 4.9 s -> 3.5 s of enumeration (gpurun_out/r2)
+    // rounds with fewer tasks than warps are bound by the latency of a lone walker: yield sooner
+    q.yield_small = (unsigned)geti("B200_ENUM_YIELD_SMALL", 8);
     q.trace     = getenv("B200_ENUM_TRACE");  // append one line per call to this file
     return q;
   }();
@@ -817,7 +816,7 @@ int run_impl(int dim, double maxdist, const double *mut_in, const double *rdiag_
   Breadth br;
   // A sharded call (one process per GPU) shares only its ROOTS between the ranks — the tasks a walker splits off later
   // stay in its own device's queue — so the roots must be fine-grained enough to balance a heavy-tailed tree on their
-  // own: with 128 roots per rank two B200 finished the 5.6e8-node BKZ-60 block no sooner than one (profiles/r2_mgpu.txt).
+  // own: with 128 roots per rank two GPUs finished the 5.6e8-node BKZ-60 block no sooner than one.
   size_t want = (size_t)tn.min_roots * (size_t)shard_world;
   if (shard_world > 1)
     want = std::max(want, (size_t)tn.shard_roots);
@@ -859,7 +858,7 @@ int run_impl(int dim, double maxdist, const double *mut_in, const double *rdiag_
   // ipc mode: ranks attached to each other push radius improvements into each other's words over NVLink.  The roots are
   // dealt round-robin in order of promise in either case: a shared ticket over the ROOTS was measured and dropped — a root
   // is split into its device's own queue after 64 nodes, so the 47 k walkers of whichever rank starts a few microseconds
-  // earlier claim every root before the other one arrives (2 ranks: 0.074 s against 0.071 s for one, profiles/r2_mgpu.txt).
+  // earlier claim every root before the other one arrives (two ranks were no faster than one).
   const bool ipc = shard_world > 1 && home->ipc_world == shard_world && home->ipc_rank == shard_rank;
   // the staged round-0 tasks of this process: its share of the roots
   std::vector<unsigned> mine;

@@ -1,7 +1,7 @@
 // fplll_matgso_shim.cpp — the reference-side binding of the device GSO: every
 //     fplll::MatGSO<Z_NR<long>,  FP_NR<double>>   (BKZ regime, bkz.cpp:812-836; wrapper small-entry stage)  and
 //     fplll::MatGSO<Z_NR<mpz_t>, FP_NR<double>>   (LLL stage 1, wrapper.cpp:538-553; the basis stays in GMP on the host)
-// object of a process runs its update_gso_row on the B200, with the UNMODIFIED libfplll and unmodified callers
+// object of a process runs its update_gso_row on the GPU, with the UNMODIFIED libfplll and unmodified callers
 // (lll.cpp, bkz.cpp, enumerate.cpp, hlll excluded, user code).
 //
 // How: fplll has no FFI for the GSO — callers hold MatGSOInterface<ZT,FT>& and read mu / r through inline accessors

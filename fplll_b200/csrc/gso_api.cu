@@ -522,7 +522,7 @@ template <class T> static int dev_alloc(b200gso *h, T **p, size_t count)
 
 extern "C" {
 
-const char *b200gso_version(void) { return "b200gso 0.1 (sm_100a)"; }
+const char *b200gso_version(void) { return "b200gso 0.1 (sm_90a)"; }
 const char *b200gso_last_error(void) { return g_err.c_str(); }
 
 int b200gso_device_count(void)
@@ -552,7 +552,7 @@ int b200gso_create(b200gso_t **out, int batch, int d, int n, int flags, int devi
   {
     // L2 -> DRAM fetch granularity hint.  The panel sweeps issue whole 256-byte lines, but the partial last panel,
     // the diagonal tiles and the scattered mu(i,.) row write touch single 32-byte sectors; at the default (128 B)
-    // those cost 9 % extra DRAM traffic (profiles/r1_update_row_v2*.txt).  B200_L2_FETCH overrides (32/64/128).
+    // those cost extra DRAM traffic.  B200_L2_FETCH overrides (32/64/128).
     const char *e = getenv("B200_L2_FETCH");
     cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, e ? (size_t)atoi(e) : (size_t)32);
   }
@@ -1035,9 +1035,10 @@ static int lll_dispatch(b200gso_t *h, int mode, double delta, double eta, int km
   long *d_stats = h->d_stats;
   int *d_st     = (int *)(h->d_stats + 4 * (size_t)S.B + 8);
   // few lattices (BKZ works on one): a whole CTA per lattice (k_lll_cta); many: one warp per lattice, the batch hides
-  // the latencies.  B200_LLL_CTA=0 forces the one-warp kernels, B200_LLL_CTA_MAX moves the switch-over.
+  // the latencies; the switch-over is two CTAs per SM.  B200_LLL_CTA=0 forces the one-warp kernels, B200_LLL_CTA_MAX moves
+  // the switch-over.
   const int cta_on  = getenv("B200_LLL_CTA") ? atoi(getenv("B200_LLL_CTA")) : 1;  // read per call: tests switch kernels
-  const int cta_max = getenv("B200_LLL_CTA_MAX") ? atoi(getenv("B200_LLL_CTA_MAX")) : 296;
+  const int cta_max = getenv("B200_LLL_CTA_MAX") ? atoi(getenv("B200_LLL_CTA_MAX")) : 2 * h->sm_count;
   const bool cta = cta_on && S.B <= cta_max && S.d > 32;
   if (cta)
   {

@@ -19,7 +19,7 @@ extern thread_local std::string b200gso_g_err;  // defined in gso_api.cu
 #define g_err b200gso_g_err
 
 constexpr int WARPS_PER_CTA = 4;
-// opt-in maximum of dynamic shared memory per CTA on sm_100: what every kernel's MaxDynamicSharedMemorySize is set to
+// opt-in maximum of dynamic shared memory per CTA on sm_90: what every kernel's MaxDynamicSharedMemorySize is set to
 constexpr int SMEM_OPTIN_MAX = 227 * 1024;
 // -DB200_LLL_PROFILE builds: device-clock phase counters of the last LLL call (b200gso_lll_profile reads them)
 extern long b200gso_g_prof[8];

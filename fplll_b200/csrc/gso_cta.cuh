@@ -1,8 +1,7 @@
 // gso_cta.cuh — CTA-cooperative pieces of the device LLL for the single-lattice (BKZ) regime.
 //
-// With one warp per lattice (gso_lll.cuh) a Babai iteration on a dim-200 basis costs ~185 us: every load is an exposed
-// L2 round trip and every dependent instruction an exposed pipeline latency (profiles/r1_lll_phase_breakdown.txt,
-// ncu: 5.4 of 10.6 cycles per issued instruction are long-scoreboard stalls, IPC 0.09).  A batch hides that behind
+// With one warp per lattice (gso_lll.cuh) a Babai iteration on a dim-200 basis is latency-bound: every load is an exposed
+// L2 round trip and every dependent instruction an exposed pipeline latency.  A batch hides that behind
 // other lattices; BKZ on ONE lattice cannot.  Here one CTA of CTA_WARPS warps serves one lattice: warp 0 (the master)
 // runs the LLL control flow of gso_lll.cuh unchanged, and the three O(kappa * d) pieces of an iteration are executed by
 // all warps as SPMD "cooperative operations", one 32-column panel per warp:

@@ -1,8 +1,8 @@
 // gso_gram.cuh — blocked recomputation of the whole float Gram matrix gf = bf * bf^T (lower triangle) for a batch.
 //
 // update_gso() row by row (k_update_gso) recomputes g(i, j) inside update_gso_row: row i re-streams the bf panels of
-// all rows j <= i, d^2 n / 64 panel-column loads per lattice (32 MB at d = 200) — measured 89 GB/s algorithmic, HBM-bound
-// on its own re-reads (profiles/r1_microbench_M1_M2_M3.txt, M2).  Here one warp produces a 32 x 32 TILE of Gram entries
+// all rows j <= i, d^2 n / 64 panel-column loads per lattice (32 MB at d = 200) — HBM-bound on its own re-reads.  Here
+// one warp produces a 32 x 32 TILE of Gram entries
 // per pass over the columns, so a bf panel column is loaded once per 32 results: this is the one piece of the path
 // that is a dense contraction (SURVEY §8 a3).
 //

@@ -3,7 +3,7 @@
 // Reference layout (fplll/gso_interface.h:548-618, nr/matrix.h:223): bf d x n, gf/mu/r d x d as
 // vector<NumVect<FP_NR<double>>> — full rectangles, one heap allocation per row.
 //
-// B200 layout, chosen for the one access pattern every hot loop shares — "lane j owns output j and walks
+// Device layout, chosen for the one access pattern every hot loop shares — "lane j owns output j and walks
 // its own row of an operand matrix in ascending column order" (update_gso_row's k-loop over mu(j,.),
 // gso_interface.cpp:147-151; get_gram's dot product over bf(j,.), numvect.h:385-395).  A plain row-major (or
 // row-packed) triangle makes that walk a 32-way strided gather.  So the two swept operands are stored as

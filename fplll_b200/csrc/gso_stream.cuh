@@ -2,8 +2,7 @@
 //
 // Same algorithm, same operation order and therefore the same bits as warp_update_gso_row (gso_warp.cuh); what changes
 // is how the two swept operands reach the SM.  The register-staged kernel (k_update_row) keeps 16 x 256 B in flight per
-// warp and is limited to 20 resident warps per SM by its staging registers: ~80 KB in flight per SM, 0.84 of the copy
-// peak (profiles/r1_update_row_ncu_summary.txt).  Here the bytes in flight live in shared memory and the TMA unit puts
+// warp and is limited to 20 resident warps per SM by its staging registers: ~80 KB in flight per SM.  Here the bytes in flight live in shared memory and the TMA unit puts
 // them there:
 //
 //   * one persistent CTA per SM of NW warps; warp c walks its own lattices (c, c + stride, ...) with the arithmetic of

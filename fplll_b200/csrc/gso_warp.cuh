@@ -99,7 +99,7 @@ __device__ inline long get_si_exp_we(double x, long &expo, long expo_add)
 // FP_NR<double>::rnd_we, nr_FP_d.inl:226-233 (rint = round-half-even).  The library form lives out of line: inlined
 // into every unrolled step of the back-substitution it made those loops ~370 instructions per step, and a lone warp
 // streaming 200 KB of straight-line code through the instruction caches per call was what the single-lattice LLL spent
-// most of its time on (profiles/r2_lll_phase_breakdown.txt: 1100 cycles per row before, the arithmetic needs ~80).
+// most of its time on.
 static __device__ __noinline__ double rnd_we_slow(double x, long expo_add)
 {
   if (fexponent(x) + expo_add >= 53)
@@ -253,7 +253,7 @@ __device__ inline void warp_stage_bf_row(const View &v, int i, int ncols, double
 // the inner loop of both dot_product (numvect.h:385-395, SUB=false) and update_gso_row (gso_interface.cpp:147-151,
 // SUB=true).  col points at this lane's row inside a panel (consecutive k are 32 doubles apart, so a warp-wide load
 // is one 256-byte line); vec lives in shared memory.  Loads are double-buffered 8 deep: the kernel is bound by HBM
-// latency x bytes in flight (profiles/), so the next group is always requested before the current one is consumed.
+// latency x bytes in flight, so the next group is always requested before the current one is consumed.
 template <bool SUB>
 __device__ inline double lane_chain(double acc, const double *__restrict__ col, const double *vec, int k0, int k1,
                                     const int cs = 32 /* column stride of the panel: 32 in HBM */)

@@ -1,4 +1,4 @@
-// hh_api.cu — B200-native MatHouseholder<long,double> (HLLL data plane) behind include/b200hh.h.
+// hh_api.cu — GPU-native MatHouseholder<long,double> (HLLL data plane) behind include/b200hh.h.
 //
 // One warp per lattice (batches are the replica axis, SURVEY §8e).  HBM layout per lattice: b (int64), bf, R, V
 // row-major d x n — update_R streams V_j[j..n) row by row (contiguous, 256-byte coalesced warp loads) against R_i held
@@ -7,7 +7,7 @@
 // Bit parity: a dot product is formed as element products in parallel (each correctly rounded, as the reference's
 // mul) followed by ONE lane adding them in ascending index order — the reference's exact chain (numvect.h:385-395).
 // In a batch the serial chain of one warp hides behind the other resident warps' HBM streaming (update_R moves
-// 16*T(i) bytes per lattice, 1.3 MB at i = 399, n = 400: ~0.5 ms of HBM time per warp, the chain is ~0.4 ms).
+// 16*T(i) bytes per lattice, 1.3 MB at i = 399, n = 400).
 #include "../../include/b200hh.h"
 #include <cstdint>
 #include <cstdio>
@@ -94,8 +94,8 @@ __device__ inline bool hsetup(const HBatch &S, HView &v, double *&sR, double *&s
 // broadcast.  The products themselves were formed one per lane (each a correctly rounded multiply).
 __device__ inline double chain_sum(const double *p, int beg, int end, int lane)
 {
-  // (a register-chunked variant — loads fetched 8 ahead of the dependent adds — measured 2x SLOWER here: the kernel is
-  // bound by how many warps fit an SM, and the extra registers halved that; gpurun_out/r2/bench_v7.json)
+  // (a register-chunked variant — loads fetched 8 ahead of the dependent adds — was slower: the kernel is bound by how
+  // many warps fit an SM, and the extra registers halved that)
   double r = 0.0;
   if (lane == 0)
   {
@@ -728,7 +728,7 @@ __global__ void hk_set_updated(HBatch S, int val)
 //
 // hk_update_R (one warp per lattice) forms every dot product V_j . R_i as per-lane products followed by ONE lane adding
 // them in the reference's order: that single-lane chain takes a full warp issue slot per add and the kernel is issue-bound
-// at 0.19 of the HBM peak (profiles/r1_enum_hh_ncu_summary.txt).  With one LATTICE per lane the 32 chains of a group of
+// far below the HBM peak.  With one LATTICE per lane the 32 chains of a group of
 // lattices advance in one instruction.  The state stays row-major per lattice (hview): the transposition is done by the
 // TMA unit — a tensor map over V (and R) seen as {flat d*n elements} x {lattice} delivers boxes of 16 consecutive elements
 // x 32 lattices (128-byte segments of 32 different rows of HBM) into shared memory with the 128-byte swizzle, which lane r
@@ -782,7 +782,7 @@ __device__ inline void x_tma_2d(void *dst, const CUtensorMap *map, int c0, int c
 }
 
 // lane r's 16 elements of a swizzled box: element k at row r, 16-byte column (k >> 1) ^ (r & 7).  (Dense 256-byte rows
-// read back with a per-lane skew were measured too — half the TMA row requests — and were slower: 2.47 against 1.77 ms.)
+// read back with a per-lane skew were tried too — half the TMA row requests — and were slower.)
 __device__ inline void x_read_box(const double *box, int lane, double (&v)[X_K])
 {
   const char *row = (const char *)box + lane * 128;
@@ -795,8 +795,7 @@ __device__ inline void x_read_box(const double *box, int lane, double (&v)[X_K])
 }
 
 // ---- one CTA per group of 32 lattices = 1 producer warp + XM_NA update warps + 1 chain warp ----
-// A single warp doing the whole sweep is bound by its own issue rate (first version: one instruction every 3.7 cycles, 0.17
-// of the HBM peak, profiles/r2_hh_x32.txt).  Here the sweep over k of pass q (reflection j = q - 2) is a pipeline of three
+// A single warp doing the whole sweep is bound by its own issue rate.  Here the sweep over k of pass q (reflection j = q - 2) is a pipeline of three
 // roles connected by mbarriers:
 //   producer  lane 0 of warp 0 walks the chunk sequence and issues the TMA boxes of chunk g into stage g % XM_S as soon
 //             as the stage is empty;
@@ -812,9 +811,8 @@ constexpr int XM_WARPS = XM_NA + 2;
 static_assert(XM_S == XM_PR, "an update warp relies on 'product slot free' implying 'TMA stage consumed'");
 // ... and the product ring must not be shorter than the number of update warps: a warp's previous chunk is XM_NA behind
 // its current one, so with XM_PR >= XM_NA the chain warp is never two rounds of a slot behind a waiting warp — a parity
-// wait can only tell adjacent phases apart.  (XM_S = 13 / XM_PR = 4 — more bytes in flight, the measured bound of this
-// kernel: 64 KB per SM against ~2.8 us per box of 32 scattered 128-byte rows — passed the small parity tests and hung at
-// n = 400 for exactly this reason; growing the ring needs XM_NA <= XM_PR <= XM_S and the shared memory for it.)
+// wait can only tell adjacent phases apart.  (XM_S = 13 / XM_PR = 4 — more bytes in flight, what bounds this kernel —
+// passed the small parity tests and hung at n = 400 for exactly this reason; growing the ring needs XM_NA <= XM_PR <= XM_S and the shared memory for it.)
 static_assert(XM_PR >= XM_NA, "product ring shorter than the number of update warps");
 
 struct XmCtl
@@ -902,8 +900,8 @@ __global__ void __launch_bounds__(XM_WARPS * 32, 1) hk_update_R_x32(HBatch S, in
   if (w == 0)
   {
     // ---- producer: lane p < XM_S owns stage p and issues the chunks g = p, p + XM_S, ... (one thread walking the whole
-    // sequence needs ~500 cycles per chunk — address arithmetic and barrier operations of a lone thread — and starved the
-    // pipeline: 1.77 ms per group; eight lanes do it eight wide) ----
+    // sequence is slowed by the address arithmetic and barrier operations of a lone thread and starved the pipeline;
+    // eight lanes do it eight wide) ----
     if (lane < XM_S)
     {
       XmIter it;
@@ -1161,8 +1159,8 @@ static void launch_update_R_h(b200hh *h, int i, int last_j)
   const HBatch &S = h->S;
   // B200_HH_X32=1 selects the lane-per-lattice kernel (default: one warp per lattice).  It needs a batch (32 lattices per
   // CTA), no R_history (its scattered per-lattice writes would cost more than the V stream) and R_i of 32 lattices in
-  // shared memory.  Measured 0.264 of the HBM peak against 0.181 for hk_update_R at one group per SM (4736 lattices) but
-  // 0.165 against 0.195 at 2960 (profiles/r2_hh_x32.txt: bound by the per-reflection hand-off), so it is not the default.
+  // shared memory.  It is faster than hk_update_R at one group per SM but slower at the batch bench.py times (bound by
+  // the per-reflection hand-off), so it is not the default.
   const char *e     = getenv("B200_HH_X32");
   const int use_x32 = e ? atoi(e) : 0;
   const size_t npad = ((size_t)S.n + X_K - 1) & ~(size_t)(X_K - 1);

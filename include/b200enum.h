@@ -1,4 +1,4 @@
-/* b200enum.h — C-ABI of the B200-native lattice enumerator (the BKZ SVP subtree search).
+/* b200enum.h — C-ABI of the GPU-native lattice enumerator (the BKZ SVP subtree search).
  *
  * Drop-in boundary: fplll's external-enumerator hook.  The reference calls a process-wide
  *   std::function<extenum_fc_enumerate>  (fplll/enum/enumerate_ext_api.h:88-92, installed with

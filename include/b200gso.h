@@ -1,4 +1,4 @@
-/* b200gso.h — C-ABI of the B200-native Gram-Schmidt (GSO) state.
+/* b200gso.h — C-ABI of the GPU-native Gram-Schmidt (GSO) state.
  *
  * Drop-in boundary for fplll's fp64 GSO hot path (SURVEY.md §8b).  The reference has no FFI: its boundary is the
  * C++ class MatGSO<Z_NR<long>, FP_NR<double>> (fplll/gso.h:33, fplll/gso_interface.h:59) whose non-virtual
@@ -79,8 +79,7 @@ int b200gso_update_gso_row(b200gso_t *h, int i, int last_j, int *ok);
 /* MatGSOInterface::update_gso, gso_interface.h:767-775 */
 int b200gso_update_gso(b200gso_t *h, int *ok);
 /* update_gso() with the whole float Gram matrix recomputed first in 32 x 32 tiles — the blocked form of get_gram
- * (gso.h:314-331) — then the row sweeps (validated on hardware in round 2: bit-exact / within 1e-9, 2-3x the row-by-row
- * form, profiles/r2_validation_queue.txt).  B200GSO_GRAM_ORDERED keeps the reference's left-to-right dot products (bit-identical state);
+ * (gso.h:314-331) — then the row sweeps (bit-exact with B200GSO_GRAM_ORDERED, within 1e-9 otherwise).  B200GSO_GRAM_ORDERED keeps the reference's left-to-right dot products (bit-identical state);
  * B200GSO_GRAM_DMMA uses fp64 tensor-core mma.m8n8k4 (identical only where every partial sum is exact). */
 #define B200GSO_GRAM_ORDERED 0
 #define B200GSO_GRAM_DMMA 1

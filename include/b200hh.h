@@ -1,4 +1,4 @@
-/* b200hh.h — C-ABI of the B200-native Householder QR state (the HLLL inner loop's data plane).
+/* b200hh.h — C-ABI of the GPU-native Householder QR state (the HLLL inner loop's data plane).
  *
  * Stands in for MatHouseholder<Z_NR<long>, FP_NR<double>> (fplll/householder.h:38, fplll/householder.cpp) with
  * HOUSEHOLDER_ROW_EXPO | HOUSEHOLDER_OP_FORCE_LONG — the object HLLLReduction drives (fplll/hlll.h:36,

@@ -9,9 +9,9 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
     config.addinivalue_line("markers", "slow: minutes per test (the reference's test_bkz over the forwarded GSO): run with "
-                                       "B200_TEST_SLOW=1; last results in profiles/r2_shim_reference_tests.txt")
+                                       "B200_TEST_SLOW=1")
     config.addinivalue_line("markers", "multigpu: needs two GPUs in one box (gpurun --gpus 2)")
 
 
@@ -24,8 +24,8 @@ def _visible_gpus():
 
 
 def pytest_collection_modifyitems(config, items):
-    """Tests that cannot run in this environment are DESELECTED (and reported as such), not skipped: the slow ones unless
-    B200_TEST_SLOW=1, the two-GPU ones on a box with fewer than two devices."""
+    """The slow tests are DESELECTED (and reported as such) unless B200_TEST_SLOW=1; the two-GPU ones are skipped on a
+    machine with fewer than two devices."""
     slow_on = bool(os.environ.get("B200_TEST_SLOW"))
     ngpu = None
     keep, drop = [], []
@@ -37,8 +37,7 @@ def pytest_collection_modifyitems(config, items):
             if ngpu is None:
                 ngpu = _visible_gpus()
             if ngpu < 2:
-                drop.append(it)
-                continue
+                it.add_marker(pytest.mark.skip(reason="needs two GPUs in one machine"))
         keep.append(it)
     if drop:
         config.hook.pytest_deselected(items=drop)

@@ -282,8 +282,95 @@ def config2_mpz_reference():
     print(rec)
 
 
+def live_fixtures():
+    """What the CPU tests once asked the reference for at run time, stored so that they run without it:
+    ref_live.npz (GSO states after seeded op scripts, Householder dump digests along an HLLL-like call sequence, HLLL
+    outputs on seeded bases), ref_islll.json (the reference's is_lll_reduced verdicts on a few bases),
+    latticegen_r_12_200*.txt (a reference-written matrix and the reference's re-save of our writer's output) and
+    strategies_default_*.json (an excerpt of strategies/default.json and digests of the whole parsed table)."""
+    import json
+    sys.path.insert(0, os.path.dirname(os.path.dirname(HERE)))
+    from fplll_b200 import io as fio
+    import test_hh_oracle as T
+    import test_oracle_golden as TG
+    arrs = {}
+    keys = ["n_known_rows", "n_known_cols", "n_source_rows", "row_expo", "gso_valid_cols", "init_row_size", "bf", "gf",
+            "mu", "r", "b"]
+    for seed, d, n, bits in TG.GSO_OPS_CASES:
+        rng = np.random.default_rng(seed)
+        b = rng.integers(-(1 << bits), 1 << bits, size=(d, n), dtype=np.int64)
+        ops = H.random_op_script(rng, d, 40)
+        s = O.RefSession(b)
+        s.lines += H.ops_to_ref_script(ops)
+        s.dump_state()
+        rec = s.run()[1][0]
+        arrs.update({"ops%d_%s" % (seed, k): rec[k] for k in keys})
+    rng = np.random.default_rng(9)
+    d = 10
+    b = np.zeros((d, d + 1), np.int64)
+    b[:, 0] = rng.integers(1, 1 << 40, size=d)
+    b[np.arange(d), np.arange(d) + 1] = 1
+    b[4] = 0
+    s = O.RefSession(b)
+    for t in range(3):
+        s.cmd("update_row %d %d" % (t, t))
+    s.dump_state()
+    s.cmd("move_row 1 9")
+    s.dump_state()
+    for t, rec in enumerate(s.run()[1]):
+        arrs.update({"ragged%d_%s" % (t, k): rec[k] for k in keys})
+    for seed, d, n, bits in T.HH_SEQ_CASES:
+        b, ops, rows_R = T.hh_call_sequence(seed, d, n, bits)
+        tmp = O.tempfile.mkdtemp(prefix="hh_")
+        mat, dump = os.path.join(tmp, "in.txt"), os.path.join(tmp, "d.bin")
+        O.write_matrix(mat, b)
+        script = ["load " + mat, "tolong", "hh 5"]
+        for op in ops:
+            script.append("hh_dump " + dump if op[0] == "dump" else
+                          "hh_" + op[0] + " " + " ".join(str(int(x)) for x in op[1:]))
+        O.run_ref("\n".join(script) + "\n")
+        arrs["hh%d_digests" % seed] = np.array([H.hh_digest(r, rows_R) for r in O.read_hh_dumps(dump)])
+    for seed, d, bits in T.HLLL_LIVE_CASES:
+        rng = np.random.default_rng(seed)
+        b = rng.integers(-(1 << bits), 1 << bits, size=(d, d), dtype=np.int64)
+        pin, pout = os.path.join(TMP, "hlll_in.txt"), os.path.join(TMP, "hlll_out.txt")
+        O.write_matrix(pin, b)
+        o = O.run_ref("load %s\ntolong\nhlll_long 0.99 0.51 0.001 0.1\nsave_long %s\n" % (pin, pout))
+        arrs["hlll%d_status" % seed] = np.int32(int(o.split("hlll_long status=")[1].split()[0]))
+        arrs["hlll%d_out" % seed] = np.array(O.read_matrix(pout), dtype=np.int64)
+    np.savez_compressed(os.path.join(HERE, "ref_live.npz"), **arrs)
+
+    # is_lll_reduced<Z_NR<mpz_t>, FP_NR<mpfr_t>> (lll.cpp:226-258) at delta 0.99, eta 0.51
+    u40, q60 = H.gold("u40_lll_long.npz"), H.gold("bkz_q60.npz")
+    swapped = u40["b_out"].copy()
+    swapped[[0, 1]] = swapped[[1, 0]]
+    verdicts = {}
+    for name, b in [("u40_b_in", u40["b_in"]), ("u40_b_out", u40["b_out"]), ("u40_b_out_rows_0_1_swapped", swapped),
+                    ("q60_b_in", q60["b_in"]), ("q60_bkz30_default_b", q60["bkz30_default_b"])]:
+        p = os.path.join(TMP, "islll.txt")
+        O.write_matrix(p, b)
+        verdicts[name] = int(O.run_ref("load %s\nislll 0.99 0.51\n" % p).split("islll ")[1].split()[0])
+    json.dump(verdicts, open(os.path.join(HERE, "ref_islll.json"), "w"), indent=1)
+
+    txt = O.latticegen(["r", 12, 200])
+    open(os.path.join(HERE, "latticegen_r_12_200.txt"), "w").write(txt)
+    p, q = os.path.join(TMP, "m.txt"), os.path.join(TMP, "m2.txt")
+    fio.write_matrix(p, fio.read_matrix(txt))
+    O.run_ref("load %s\nsave %s\n" % (p, q))
+    open(os.path.join(HERE, "latticegen_r_12_200_resaved.txt"), "w").write(open(q).read())
+
+    src = os.path.join(os.path.dirname(os.path.dirname(HERE)), "oracle", "_ref", "strategies", "default.json")
+    table = fio.load_strategies_json(src)
+    json.dump({str(bs): H.strategy_digest(v) for bs, v in sorted(table.items())},
+              open(os.path.join(HERE, "strategies_default_digests.json"), "w"), indent=0)
+    excerpt = [e for e in json.load(open(src)) if e["block_size"] in (0, 1, 2, 10, 20)]
+    json.dump(excerpt, open(os.path.join(HERE, "strategies_default_excerpt.json"), "w"), separators=(",", ":"))
+
+
 if __name__ == "__main__":
-    if "--config2" in sys.argv:
+    if "--live" in sys.argv:
+        live_fixtures()
+    elif "--config2" in sys.argv:
         config2_mpz_reference()
     elif "--dual" in sys.argv:
         enum_dual_subsol_fixtures()

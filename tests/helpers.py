@@ -10,6 +10,12 @@ def gold(name):
     return np.load(os.path.join(GOLD, name), allow_pickle=False)
 
 
+def gold_json(name):
+    import json
+    with open(os.path.join(GOLD, name)) as f:
+        return json.load(f)
+
+
 def bits(a):
     return np.ascontiguousarray(a, dtype=np.float64).view(np.int64)
 
@@ -41,6 +47,72 @@ def assert_state_equal(got, ref, what="", check_b=True):
         assert eq_f64(got["gf"][i, : i + 1], ref["gf"][i, : i + 1]), "%s gf row %d" % (what, i)
         assert eq_f64(got["mu"][i, : min(v, i)], ref["mu"][i, : min(v, i)]), "%s mu row %d" % (what, i)
         assert eq_f64(got["r"][i, :v], ref["r"][i, :v]), "%s r row %d" % (what, i)
+
+
+def _f64_bytes(a):
+    """float64 bytes with every NaN in one canonical encoding (eq_f64's NaN == NaN, any payload)."""
+    a = np.array(a, dtype=np.float64)
+    a[np.isnan(a)] = np.nan
+    return a.tobytes()
+
+
+def hh_digest(s, rows_R):
+    """sha256 over the MatHouseholder state entries test_hh_oracle compares: metadata, integer arrays, the first rows_R
+    rows of sigma / norm_square_b / bf / R and the known rows of V (bit patterns, NaN canonical)."""
+    import hashlib
+    h = hashlib.sha256()
+    nk = int(s["n_known_rows"])
+    h.update(np.array([nk, int(s["n_known_cols"])], np.int64).tobytes())
+    for k in ["row_expo", "expo_norm_square_b", "b"]:
+        h.update(np.ascontiguousarray(s[k], np.int64).tobytes())
+    for k in ["sigma", "norm_square_b", "bf", "R"]:
+        h.update(_f64_bytes(s[k][:rows_R]))
+    h.update(_f64_bytes(s["V"][:nk]))
+    return h.hexdigest()
+
+
+def strategy_digest(entry):
+    """sha256 of one block size's (preprocessing, gh_factor, expectation, coefficients) arrays."""
+    import hashlib
+    h = hashlib.sha256()
+    pp, gh, ex, coef = entry
+    h.update(np.asarray(pp, np.int32).tobytes())
+    for a in (gh, ex, coef):
+        h.update(np.array(a.shape, np.int64).tobytes() + _f64_bytes(a))
+    return h.hexdigest()
+
+
+def is_lll_reduced(b, delta=0.99, eta=0.51):
+    """The test of is_lll_reduced (lll.cpp:226-258) in exact arithmetic: |mu(i,j)| <= eta for all j < i and
+    r(i,i) >= (delta - mu(i,i-1)^2) r(i-1,i-1).  Integral Gram-Schmidt (Cohen, Algorithm 2.6.7): dd[i+1] = r(0,0)
+    ... r(i,i) and lam[i][j] = dd[j+1] mu(i,j) are integers.  tests/golden/ref_islll.json pins it to the reference."""
+    from fractions import Fraction
+    b = [[int(x) for x in row] for row in np.asarray(b)]
+    d = len(b)
+    dd = [1] + [0] * d
+    lam = [[0] * d for _ in range(d)]
+    for i in range(d):
+        for j in range(i + 1):
+            u = sum(x * y for x, y in zip(b[i], b[j]))
+            for k in range(j):
+                u = (dd[k + 1] * u - lam[i][k] * lam[j][k]) // dd[k]
+            if j < i:
+                lam[i][j] = u
+            else:
+                dd[i + 1] = u
+        if dd[i + 1] == 0:
+            raise ValueError("rows are linearly dependent")
+    e, de = Fraction(eta), Fraction(delta)
+    for i in range(d):
+        for j in range(i):
+            if abs(Fraction(lam[i][j], dd[j + 1])) > e:
+                return False
+    for i in range(1, d):
+        mu = Fraction(lam[i][i - 1], dd[i])
+        r_prev, r_i = Fraction(dd[i], dd[i - 1]), Fraction(dd[i + 1], dd[i])
+        if r_i < (de - mu * mu) * r_prev:
+            return False
+    return True
 
 
 def lattice_state(st, l):

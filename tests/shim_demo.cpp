@@ -1,7 +1,7 @@
 // shim_demo — TEST PROGRAM: the reference's own LLLReduction over its own MatGSO, compiled against the unmodified
 // reference headers and linked with the unmodified libfplll.so.  Run once plainly and once with
 // LD_PRELOAD=libb200fplll.so (fplll_b200/csrc/fplll_matgso_shim.cpp): the second run executes every update_gso_row on
-// the B200 and must print byte-identical results (the device GSO is bit-exact, so LLL walks the same trajectory).
+// the GPU and must print byte-identical results (the device GSO is bit-exact, so LLL walks the same trajectory).
 // usage: shim_demo IN.txt long|mpz|long_gram|mpz_gram OUT.bin     (_gram: GSO_INT_GRAM, the exact integer Gram matrix)
 #include <fplll/fplll.h>
 #include <cstdio>

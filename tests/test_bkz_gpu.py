@@ -57,16 +57,21 @@ def test_bkz_default_strategies_same_status_and_quality(fb, tag, bs):
     assert abs(s_got - s_ref) < 0.15 * abs(s_ref), (s_got, s_ref)
 
 
-@pytest.mark.skipif(not O.have_ref(), reason="oracle/_ref not shipped")
-def test_bkz_output_is_lll_reduced_by_the_reference_checker(fb, tmp_path):
-    z = H.gold("bkz_q60.npz")
+def test_bkz_output_is_lll_reduced_by_the_reference_checker(fb):
+    """is_lll_reduced (lll.cpp:226-258) in exact arithmetic (helpers.py), first checked against the reference's own
+    verdicts on fixed bases (tests/golden/ref_islll.json), then on the device BKZ output."""
+    u40, z = H.gold("u40_lll_long.npz"), H.gold("bkz_q60.npz")
+    swapped = u40["b_out"].copy()
+    swapped[[0, 1]] = swapped[[1, 0]]
+    verdicts = H.gold_json("ref_islll.json")
+    for name, basis in [("u40_b_in", u40["b_in"]), ("u40_b_out", u40["b_out"]), ("u40_b_out_rows_0_1_swapped", swapped),
+                        ("q60_b_in", z["b_in"]), ("q60_bkz30_default_b", z["bkz30_default_b"])]:
+        assert H.is_lll_reduced(basis, 0.99, 0.51) == bool(verdicts[name]), name
     b = z["b_in"].copy()
     st, _ = fb.bkz_reduction(b, fb.BKZParam(30, strategies="default", flags=fb.BKZ_NO_LLL | fb.BKZ_MAX_LOOPS,
                                             max_loops=1))
     assert st == 8
-    p = tmp_path / "out.txt"
-    O.write_matrix(str(p), b)
-    assert "islll 1" in O.run_ref("load %s\nislll 0.99 0.51\n" % p)
+    assert H.is_lll_reduced(b, 0.99, 0.51)
 
 
 def test_bkz_reports_a_failing_preliminary_lll_as_status(fb):

@@ -102,8 +102,8 @@ def test_reference_bkz_with_the_plugin_installed(tmp_path):
 @pytest.mark.multigpu
 def test_two_devices_in_one_process_visit_the_same_nodes(en):
     """b200enum_run(devices = [0, 1]): subtree roots dealt over two GPUs of the box from ONE process (what the BKZ driver
-    does with `devices`); fixed radius, so the per-level node counts must equal the oracle's.  Needs two GPUs (deselected
-    on a one-GPU box, tests/conftest.py; last run: gpurun --gpus 2, profiles/r2_mgpu.txt)."""
+    does with `devices`); fixed radius, so the per-level node counts must equal the oracle's.  Needs two GPUs (skipped
+    on a one-GPU machine, tests/conftest.py)."""
     # a call this small stays on the first device (hand-off threshold B200_ENUM_FAN_NODES, 200 M nodes) ...
     z = H.gold("enum_r200_b30_unpruned.npz")
     R = 0.55 * float(z["maxdist"])

@@ -1,8 +1,6 @@
 """CPU tests (no GPU): the C restatement of MatHouseholder<long,double> (oracle/hh_oracle.c) against the UNMODIFIED
-reference driven call by call through oracle/_ref/ref_probe (bit-exact), plus the reference's own test_householder
+reference driven call by call through oracle/_ref/ref_probe (bit-exact; its results are stored under tests/golden), plus the reference's own test_householder
 relation (tests/test_gso.cpp:101-152): mu(i,j) = R(i,j)/R(j,j) and r(i,j) = R(i,j)*R(j,j) against the GSO."""
-import os
-
 import numpy as np
 import pytest
 
@@ -10,40 +8,13 @@ import helpers as H
 from oracle import oracle as O
 
 
-def _run_both(b, ops, flags=5):
-    tmp = O.tempfile.mkdtemp(prefix="hh_")
-    mat, dump = os.path.join(tmp, "in.txt"), os.path.join(tmp, "d.bin")
-    O.write_matrix(mat, b)
-    script = ["load " + mat, "tolong", "hh %d" % flags]
-    m = O.OracleHouseholder(b, flags)
-    states = []
-    for op in ops:
-        if op[0] == "dump":
-            script.append("hh_dump " + dump)
-            states.append(m.state())
-        else:
-            script.append("hh_" + op[0] + " " + " ".join(str(int(x)) for x in op[1:]))
-            getattr(m, op[0])(*op[1:])
-    O.run_ref("\n".join(script) + "\n")
-    return states, O.read_hh_dumps(dump)
+HH_SEQ_CASES = [(1, 10, 10, 20), (2, 24, 30, 12), (3, 40, 40, 30)]
 
 
-def _assert_same(s, r, rows_R, what):
-    nk = r["n_known_rows"]
-    assert s["n_known_rows"] == nk and s["n_known_cols"] == r["n_known_cols"], what
-    for k in ["row_expo", "expo_norm_square_b", "b"]:
-        assert np.array_equal(s[k], r[k]), what + " " + k
-    for k in ["sigma", "norm_square_b", "bf"]:
-        assert H.eq_f64(s[k][:rows_R], r[k][:rows_R]), what + " " + k
-    assert H.eq_f64(s["R"][:rows_R], r["R"][:rows_R]), what + " R"
-    assert H.eq_f64(s["V"][:nk], r["V"][:nk]), what + " V"
-
-
-@pytest.mark.skipif(not O.have_ref(), reason="oracle/_ref not built")
-@pytest.mark.parametrize("seed,d,n,bits", [(1, 10, 10, 20), (2, 24, 30, 12), (3, 40, 40, 30)])
-def test_hlll_like_call_sequence_live_vs_reference(seed, d, n, bits):
+def hh_call_sequence(seed, d, n, bits):
     """refresh_R_bf / update_R / size_reduce (with integer + float row operations) / swap / recover_R in the order
-    HLLLReduction::hlll issues them (hlll.cpp:49-171) on an UNREDUCED random basis."""
+    HLLLReduction::hlll issues them (hlll.cpp:49-171) on an UNREDUCED random basis; returns (basis, ops, rows of R
+    that are defined at every dump)."""
     rng = np.random.default_rng(seed)
     b = rng.integers(-(1 << bits), 1 << bits, size=(d, n), dtype=np.int64)
     ops = [("refresh_R_bf", 0), ("update_R_last", 0), ("refresh_R_bf", 1)]
@@ -62,10 +33,25 @@ def test_hlll_like_call_sequence_live_vs_reference(seed, d, n, bits):
             k -= 1
             ops += [("recover_R", k), ("dump",), ("set_updated_R_false",)]
     ops.append(("dump",))
-    states, recs = _run_both(b, ops)
-    assert len(states) == len(recs) > 5
-    for t, (s, r) in enumerate(zip(states, recs)):
-        _assert_same(s, r, min(d, kmax + 1), "seed %d dump %d" % (seed, t))
+    return b, ops, min(d, kmax + 1)
+
+
+@pytest.mark.parametrize("seed,d,n,bits", HH_SEQ_CASES)
+def test_hlll_like_call_sequence_live_vs_reference(seed, d, n, bits):
+    """the call sequence of hh_call_sequence on the oracle, bit-exact against the reference's state at every dump
+    (digests of the reference's dumps in tests/golden/ref_live.npz, make_golden.py --live)."""
+    b, ops, rows_R = hh_call_sequence(seed, d, n, bits)
+    m = O.OracleHouseholder(b, 5)
+    states = []
+    for op in ops:
+        if op[0] == "dump":
+            states.append(m.state())
+        else:
+            getattr(m, op[0])(*op[1:])
+    want = H.gold("ref_live.npz")["hh%d_digests" % seed]
+    assert len(states) == len(want) > 5
+    for t, s in enumerate(states):
+        assert H.hh_digest(s, rows_R) == want[t], "seed %d dump %d" % (seed, t)
 
 
 def test_householder_relation_with_gso():
@@ -101,17 +87,15 @@ def test_oracle_hlll_equals_reference_golden(tag):
     assert np.array_equal(m.state()["b"], g[tag + "_out"])
 
 
-@pytest.mark.skipif(not O.have_ref(), reason="oracle/_ref not built")
-@pytest.mark.parametrize("seed,d,bits", [(5, 30, 25), (6, 50, 12), (7, 70, 40)])
+HLLL_LIVE_CASES = [(5, 30, 25), (6, 50, 12), (7, 70, 40)]
+
+
+@pytest.mark.parametrize("seed,d,bits", HLLL_LIVE_CASES)
 def test_oracle_hlll_live_vs_reference(seed, d, bits):
-    """same, on seeded random bases, against the reference run live (status and output basis)."""
+    """same, on seeded random bases, against the reference's status and output basis (tests/golden/ref_live.npz)."""
     rng = np.random.default_rng(seed)
     b = rng.integers(-(1 << bits), 1 << bits, size=(d, d), dtype=np.int64)
-    tmp = O.tempfile.mkdtemp(prefix="hlll_")
-    pin, pout = os.path.join(tmp, "in.txt"), os.path.join(tmp, "out.txt")
-    O.write_matrix(pin, b)
-    o = O.run_ref("load %s\ntolong\nhlll_long 0.99 0.51 0.001 0.1\nsave_long %s\n" % (pin, pout))
-    rst = int(o.split("hlll_long status=")[1].split()[0])
+    z = H.gold("ref_live.npz")
     m = O.OracleHouseholder(b)
-    assert m.hlll() == rst
-    assert np.array_equal(m.state()["b"], np.array(O.read_matrix(pout), dtype=np.int64))
+    assert m.hlll() == int(z["hlll%d_status" % seed])
+    assert np.array_equal(m.state()["b"], z["hlll%d_out" % seed])

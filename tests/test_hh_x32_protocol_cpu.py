@@ -1,7 +1,7 @@
 """CPU model check of the synchronisation protocol of hk_update_R_x32 (fplll_b200/csrc/hh_api.cu): producer lanes, update
 warps and the chain warp talk through mbarriers whose waits only see the PARITY of a phase, so a waiter that falls two
 completions behind (or runs two ahead) of a barrier passes or blocks wrongly.  That is not a theoretical worry: a ring of 13
-TMA stages with 4 product slots passed the small GPU parity tests and hung at n = 400 (profiles/r2_hh_x32.txt).
+TMA stages with 4 product slots passed the small GPU parity tests and hung at n = 400.
 
 The model below replays the kernel's three loops as coroutines over the same chunk sequence (XmIter), with the barrier
 semantics of PTX (`mbarrier.try_wait.parity P` succeeds iff the phase in progress has the other parity; a count-1 barrier
@@ -162,6 +162,6 @@ def test_the_model_finds_the_configuration_that_hung_on_the_gpu():
 
 @pytest.mark.parametrize("NA,S,PR", [(6, 12, 6), (4, 13, 4), (6, 8, 8)])
 def test_deeper_rings_that_respect_the_constraint_are_safe(NA, S, PR):
-    """the next step of profiles/r2_hh_x32.txt (more bytes in flight) within XM_NA <= XM_PR <= XM_S"""
+    """more bytes in flight than the shipped ring, within XM_NA <= XM_PR <= XM_S"""
     for seed in range(15):
         assert simulate(400, 10, NA, S, PR, 16, seed) > 0

@@ -1,31 +1,31 @@
 """CPU tests of the reference's text formats (fplll_b200/io.py, SURVEY §8 f3): matrices written by the reference's own
-latticegen / read back by its own CLI, strategies/default.json against the committed array form, the GSO dump record."""
+latticegen / read back by its own reader (stored under tests/golden), strategies/default.json against the committed
+array form, the GSO dump record."""
 import json
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
 from fplll_b200 import io as fio
-from oracle import oracle as O
+import helpers as H
 
 HERE = os.path.dirname(os.path.abspath(__file__))
+GOLD = os.path.join(HERE, "golden")
 
 
-@pytest.mark.skipif(not O.have_ref(), reason="oracle/_ref not built")
 def test_matrix_text_format_round_trips_through_the_reference(tmp_path):
-    txt = O.latticegen(["r", 12, 200])          # 12 x 13, 200-bit entries: written by Matrix<T>::print
+    # written by the reference's own latticegen (Matrix<T>::print): `latticegen r 12 200`, 12 x 13, 200-bit entries
+    txt = open(os.path.join(GOLD, "latticegen_r_12_200.txt")).read()
     a = fio.read_matrix(txt)
     assert a.shape == (12, 13) and int(a[0, 0]).bit_length() > 64
     p = str(tmp_path / "m.txt")
     fio.write_matrix(p, a)
-    # the reference's own reader accepts our output and prints it back identically (fplll -a lll -l 0 would reduce; use
-    # ref_probe's load/save pair: Matrix<T>::read then print)
-    q = str(tmp_path / "m2.txt")
-    O.run_ref("load %s\nsave %s\n" % (p, q))
+    # the reference's own reader accepted our output and printed it back identically (ref_probe's load/save pair:
+    # Matrix<T>::read then print, tests/golden/make_golden.py --live)
+    q = os.path.join(GOLD, "latticegen_r_12_200_resaved.txt")
     assert np.array_equal(fio.read_matrix(q), a)
-    assert open(q).read().split() == fio.write_matrix(None, a).split()
+    assert open(q).read().split() == open(p).read().split() == fio.write_matrix(None, a).split()
 
 
 def test_read_matrix_pads_short_rows_and_refuses_overflow():
@@ -36,13 +36,16 @@ def test_read_matrix_pads_short_rows_and_refuses_overflow():
 
 
 def test_strategies_json_equals_the_committed_table():
-    ref = os.path.join(os.path.dirname(HERE), "oracle", "_ref", "strategies", "default.json")
-    if not os.path.exists(ref):
-        pytest.skip("strategies/default.json not shipped")
-    got = fio.load_strategies_json(ref)
+    """the committed table (fplll_b200/data) is the reference's strategies/default.json: every block size's arrays hash
+    like the reference file's parsed with load_strategies_json, and the parser reads an excerpt of that file."""
     from fplll_b200.bkz import load_strategies
     want = load_strategies()
-    assert sorted(got) == sorted(want)
+    digests = json.load(open(os.path.join(GOLD, "strategies_default_digests.json")))
+    assert sorted(int(bs) for bs in digests) == sorted(want)
+    for bs in want:
+        assert H.strategy_digest(want[bs]) == digests[str(bs)], bs
+    got = fio.load_strategies_json(os.path.join(GOLD, "strategies_default_excerpt.json"))
+    assert sorted(got) == [0, 1, 2, 10, 20]
     for bs in got:
         for x, y in zip(got[bs], want[bs]):
             assert np.array_equal(np.asarray(x), np.asarray(y)), bs

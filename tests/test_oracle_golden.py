@@ -58,41 +58,33 @@ def test_lll_u40_matches_reference_basis():
     assert np.array_equal(m.state()["b"], z["b_out"])
 
 
-@pytest.mark.skipif(not O.have_ref(), reason="oracle/_ref not built")
-@pytest.mark.parametrize("seed,d,n,bits", [(1, 12, 12, 20), (2, 33, 40, 30), (3, 64, 65, 12), (4, 7, 9, 50)])
+GSO_OPS_CASES = [(1, 12, 12, 20), (2, 33, 40, 30), (3, 64, 65, 12), (4, 7, 9, 50)]
+
+
+@pytest.mark.parametrize("seed,d,n,bits", GSO_OPS_CASES)
 def test_random_ops_live_vs_reference(seed, d, n, bits):
+    """a seeded random op script; the reference's state after it is in tests/golden/ref_live.npz (make_golden.py --live)."""
     rng = np.random.default_rng(seed)
     b = rng.integers(-(1 << bits), 1 << bits, size=(d, n), dtype=np.int64)
     ops = H.random_op_script(rng, d, 40)
-    s = O.RefSession(b)
-    s.lines += H.ops_to_ref_script(ops)
-    s.dump_state()
-    _, recs = s.run()
     m = O.OracleGSO(b)
     H.apply_ops(m, ops)
-    H.assert_state_equal(m.state(), recs[0], "seed %d" % seed)
+    H.assert_state_equal(m.state(), _state_from_npz(H.gold("ref_live.npz"), "ops%d_" % seed), "seed %d" % seed)
 
 
-@pytest.mark.skipif(not O.have_ref(), reason="oracle/_ref not built")
 def test_ragged_and_zero_rows_live():
-    """knapsack-style identity tail (n_known_cols grows with discover_row) and an all-zero row (LLL parks it)."""
+    """knapsack-style identity tail (n_known_cols grows with discover_row) and an all-zero row (LLL parks it); the
+    reference's two states are in tests/golden/ref_live.npz."""
     rng = np.random.default_rng(9)
     d = 10
     b = np.zeros((d, d + 1), np.int64)
     b[:, 0] = rng.integers(1, 1 << 40, size=d)
     b[np.arange(d), np.arange(d) + 1] = 1
     b[4] = 0
-    s = O.RefSession(b)
-    s.cmd("update_row 0 0")
-    s.cmd("update_row 1 1")
-    s.cmd("update_row 2 2")
-    s.dump_state()
-    s.cmd("move_row 1 9")
-    s.dump_state()
-    _, recs = s.run()
+    z = H.gold("ref_live.npz")
     m = O.OracleGSO(b)
     for t in range(3):
         m.update_gso_row(t, t)
-    H.assert_state_equal(m.state(), recs[0], "partial")
+    H.assert_state_equal(m.state(), _state_from_npz(z, "ragged0_"), "partial")
     m.move_row(1, 9)
-    H.assert_state_equal(m.state(), recs[1], "after move_row beyond known rows")
+    H.assert_state_equal(m.state(), _state_from_npz(z, "ragged1_"), "after move_row beyond known rows")

@@ -1,7 +1,7 @@
 """GPU tests of the MatGSO forwarding shim (fplll_b200/csrc/fplll_matgso_shim.cpp, SURVEY §8 b1 / N2): the UNMODIFIED
 reference library and its unmodified callers (LLLReduction, BKZReduction, the reference's own test programs) run
 with libb200fplll.so preloaded, so every MatGSO<Z_NR<long>|Z_NR<mpz_t>, FP_NR<double>>::update_gso_row executes on the
-B200.  The device GSO is bit-exact, so results must be byte-identical to the plain runs."""
+GPU.  The device GSO is bit-exact, so results must be byte-identical to the plain runs."""
 import os
 import subprocess
 
@@ -93,8 +93,8 @@ def test_config2_lll_on_r200_2000_in_the_mpz_regime_fails_exactly_like_the_refer
     assert sha(out) == ref["out_bin_sha256"], "mu / r / row_expo after the failing LLL differ"
 
 
-# the reference's test_bkz takes 4-5 minutes per run with every update_gso_row forwarded (260 s measured,
-# profiles/r2_shim_reference_tests.txt): deselected unless B200_TEST_SLOW=1 (tests/conftest.py)
+# the reference's test_bkz takes minutes per run with every update_gso_row forwarded: deselected unless B200_TEST_SLOW=1
+# (tests/conftest.py)
 _SLOW = pytest.mark.slow
 
 

@@ -1,4 +1,4 @@
-"""SURVEY §8(d) micro-benchmarks M1 / M2 / M3 of the device GSO (run on a B200:  python tools/microbench.py > out.txt).
+"""SURVEY §8(d) micro-benchmarks M1 / M2 / M3 of the device GSO (run on an H100:  python tools/microbench.py > out.txt).
 
   M1  per-call update_gso_row(i, i), i in {39, 199, 399}, Gram row invalid (g=1) and valid (g=0): one lattice (the
       latency of a single call, what a per-call forwarder would pay) and a full batch (2 x resident warps).

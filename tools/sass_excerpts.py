@@ -1,6 +1,6 @@
 """Static SASS evidence of the hot kernels: per-kernel opcode histogram + a few lines around the instructions that matter
 (UTMALDG / UBLKCP / SYNCS = TMA + mbarrier, DMMA = fp64 tensor core, ATOMG / REDG .SYS = peer atomics).
-usage: python tools/sass_excerpts.py > profiles/rN_sass_excerpts.txt   (needs cuobjdump; no GPU)"""
+usage: python tools/sass_excerpts.py > sass_excerpts.txt   (needs cuobjdump; no GPU)"""
 import collections
 import re
 import subprocess

@@ -1,6 +1,6 @@
-// ubench_lat.cu — dependent-issue latencies that bound the single-lattice LLL chains on B200 (one warp, clock64):
+// ubench_lat.cu — dependent-issue latencies that bound the single-lattice LLL chains on the GPU (one warp, clock64):
 // fp64 add / mul / sub chains, the shuffle-multiply-subtract step of the triangular solves, shared / L2 loads,
-// named and cluster barriers, DSMEM.  Build: nvcc -gencode arch=compute_100a,code=sm_100a --fmad=false -O3 -o ubench_lat
+// named and cluster barriers, DSMEM.  Build: nvcc -gencode arch=compute_90a,code=sm_90a --fmad=false -O3 -o ubench_lat
 #include <cooperative_groups.h>
 #include <cstdio>
 #include <cuda_runtime.h>

@@ -1,11 +1,11 @@
-// ubench_read.cu — what can a read-mostly kernel pull out of HBM on this B200?  The roofline denominator of bench.py is
+// ubench_read.cu — what can a read-mostly kernel pull out of HBM on this GPU?  The roofline denominator of bench.py is
 // the driver's COPY bandwidth (MEASURED_PEAKS.json: read + write bytes of a device-to-device copy); update_gso_row is
 // read-only, and its reads are 2960 concurrent streams (one per lattice) of 256-byte lines rather than one linear sweep.
 //   mode 0: linear sweep, every thread 16-byte loads, grid-stride (the friendliest pattern there is)
 //   mode 1: one stream per warp: warp w reads its own contiguous region of `per` bytes in 256-byte lines, 16 lines in
 //           flight per warp, 20 warps per SM (k_update_row's geometry: 5920 lattices x 485 KB)
 //   mode 2: as 1 with 40 lines in flight per warp
-// build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o ubench_read tools/ubench_read.cu
+// build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o ubench_read tools/ubench_read.cu
 #include <cstdio>
 #include <cstdlib>
 #include <cuda_runtime.h>
@@ -63,7 +63,7 @@ int main()
     {
       cudaEventRecord(e0);
       if (mode == 0)
-        k_linear<<<148 * 16, 256>>>((const double2 *)buf, bytes / 16, out);
+        k_linear<<<132 * 16, 256>>>((const double2 *)buf, bytes / 16, out);
       else if (mode == 1)
         k_streams<16><<<(nstreams + 3) / 4, 128>>>(buf, per / 8, nstreams, out);
       else
