@@ -10,6 +10,7 @@ from .gso import MatGSO, lll_reduction, GSO_DEFAULT, GSO_ROW_EXPO, GSO_OP_FORCE_
 from .gso import RED_SUCCESS, RED_GSO_FAILURE, RED_BABAI_FAILURE, RED_LLL_FAILURE  # noqa: F401
 from .bkz import BKZParam, bkz_reduction, load_strategies  # noqa: F401
 from .bkz import BKZ_DEFAULT, BKZ_VERBOSE, BKZ_NO_LLL, BKZ_MAX_LOOPS, BKZ_AUTO_ABORT, BKZ_GH_BND, BKZ_SHRINK_RADIUS  # noqa: F401
+from .bkz import BKZ_MAX_TIME, BKZ_BOUNDED_LLL, BKZ_SD_VARIANT, BKZ_SLD_RED  # noqa: F401
 from .householder import MatHouseholder, hlll_reduction  # noqa: F401
 from .enumeration import enumerate_svp  # noqa: F401
 from .io import read_matrix, write_matrix, load_strategies_json, GSODump  # noqa: F401

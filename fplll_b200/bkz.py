@@ -9,6 +9,7 @@ from ._lib import B200Error, load
 
 BKZ_DEFAULT, BKZ_VERBOSE, BKZ_NO_LLL, BKZ_MAX_LOOPS, BKZ_MAX_TIME = 0, 1, 2, 4, 8  # defs.h:264-274
 BKZ_BOUNDED_LLL, BKZ_AUTO_ABORT, BKZ_GH_BND = 0x10, 0x20, 0x80
+BKZ_SD_VARIANT, BKZ_SLD_RED = 0x100, 0x200  # self-dual BKZ, slide reduction (mutually exclusive)
 BKZ_SHRINK_RADIUS = 0x10000  # include/b200bkz.h: not a reference flag (order-dependent enumeration like the reference's)
 RED_BKZ_FAILURE, RED_BKZ_TIME_LIMIT, RED_BKZ_LOOPS_LIMIT = 6, 7, 8
 _P = C.POINTER
@@ -74,7 +75,7 @@ class BKZParam:
 
 def bkz_reduction(b, param, devices=None):
     """bkz_reduction(ZZ_mat<long>& b, BKZParam) in the int64 regime (bkz.cpp:812-836): reduces the (d, n) int64 numpy
-    array IN PLACE.  Returns (RedStatus, stats dict).  param.strategies: None (EmptyStrategy for every block size),
+    array IN PLACE.  BKZ 2.0 by default, self-dual BKZ with BKZ_SD_VARIANT, slide reduction with BKZ_SLD_RED.  Returns (RedStatus, stats dict).  param.strategies: None (EmptyStrategy for every block size),
     "default" (the reference's strategies/default.json table) or a dict as returned by load_strategies."""
     L = _lib()
     arr = np.ascontiguousarray(b, dtype=np.int64)

@@ -1,4 +1,4 @@
-// bkz_api.cu — host control flow of BKZ 2.0 over the device GSO / LLL (b200gso.h) and the device enumerator
+// bkz_api.cu — host control flow of BKZ 2.0, SD-BKZ and slide reduction over the device GSO / LLL (b200gso.h) and the device enumerator
 // (b200enum.h).  Mirrors BKZReduction<Z_NR<long>, FP_NR<double>> (fplll/bkz.cpp) method for method; every method
 // names the reference lines it restates.  Nothing here computes a Gram-Schmidt coefficient on the CPU: the host only
 // decides which block, which radius and which pruning vector, and replays the enumeration result as row operations.
@@ -89,7 +89,7 @@ public:
   int enum_flags = 0;
 
   // ---- thin wrappers over the device GSO -------------------------------------------------------------
-  void lll(int kmin, int kstart, int kend, long *n_swaps)
+  void lll(int kmin, int kstart, int kend, long *n_swaps, bool check = true)
   {
     const double t0 = now_s();
     int status      = 0;
@@ -108,7 +108,7 @@ public:
 #endif
     if (n_swaps)
       *n_swaps = stats[0];
-    if (status != 0)
+    if (status != 0 && check)
       throw RedFailure{status};  // the reference throws runtime_error(RED_STATUS_STR[status]), bkz.cpp:109-112
   }
   void size_reduction(int kmin, int kend, int sr_start = 0)
@@ -266,8 +266,9 @@ public:
     return clean;
   }
 
-  // svp_postprocessing, bkz.cpp:128-203 (primal)
-  void svp_postprocessing(int kappa, int block_size, const std::vector<double> &solution)
+  // svp_postprocessing, bkz.cpp:128-203.  Dual: the solution is a dual vector; the row operations are the transposed
+  // inverses of the primal ones and the new vector lands at the END of the block (pos = kappa + block_size - 1).
+  void svp_postprocessing(int kappa, int block_size, const std::vector<double> &solution, bool dual)
   {
     int nz_vectors = 0, i_vector = -1;
     for (int i = block_size - 1; i >= 0; i--)
@@ -277,25 +278,36 @@ public:
         if (i_vector == -1 && fabs(solution[i]) == 1)
           i_vector = i;
       }
-    const int pos = kappa;
+    const int pos = dual ? kappa + block_size - 1 : kappa;
     if (nz_vectors == 1)
       move_row(kappa + i_vector, pos);
     else if (i_vector != -1)
     {
-      const int sol_i = (int)solution[i_vector];
+      int sol_i = (int)solution[i_vector];
+      if (dual)
+        sol_i *= -1;
       for (int i = 0; i < block_size; ++i)
         if (solution[i] != 0 && i != i_vector)
-          row_addmul(kappa + i_vector, kappa + i, sol_i * solution[i]);
-      row_op_end(kappa + i_vector, kappa + i_vector + 1);
+        {
+          if (dual)
+            row_addmul(kappa + i, kappa + i_vector, sol_i * solution[i]);
+          else
+            row_addmul(kappa + i_vector, kappa + i, sol_i * solution[i]);
+        }
+      if (dual)
+        row_op_end(kappa, kappa + block_size);
+      else
+        row_op_end(kappa + i_vector, kappa + i_vector + 1);
       move_row(kappa + i_vector, pos);
     }
     else
-      svp_postprocessing_generic(kappa, block_size, solution);
+      svp_postprocessing_generic(kappa, block_size, solution, dual);
     flush();
   }
 
-  // svp_postprocessing_generic, bkz.cpp:205-272 (primal): tree-based gcd on the coefficient vector
-  void svp_postprocessing_generic(int kappa, int block_size, const std::vector<double> &solution)
+  // svp_postprocessing_generic, bkz.cpp:205-272: tree-based gcd on the coefficient vector (dual: row_sub in the other
+  // direction, and the vector is already where it belongs, at the end of the block)
+  void svp_postprocessing_generic(int kappa, int block_size, const std::vector<double> &solution, bool dual)
   {
     std::vector<double> x = solution;
     const int dd          = block_size;
@@ -323,7 +335,10 @@ public:
             while (x[k - off] <= x[k])
             {
               x[k] = x[k] - x[k - off];
-              row_addmul(kappa + k - off, kappa + k, 1.0);  // row_add(kappa + k - off, kappa + k)
+              if (dual)
+                row_addmul(kappa + k, kappa + k - off, -1.0);  // row_sub(kappa + k, kappa + k - off)
+              else
+                row_addmul(kappa + k - off, kappa + k, 1.0);  // row_add(kappa + k - off, kappa + k)
             }
             std::swap(x[k], x[k - off]);
             row_swap(kappa + k - off, kappa + k);
@@ -334,13 +349,15 @@ public:
       off *= 2;
     }
     row_op_end(kappa, kappa + dd);
-    move_row(kappa + dd - 1, kappa);
+    if (!dual)
+      move_row(kappa + dd - 1, kappa);
   }
 
-  // svp_reduction, bkz.cpp:274-358 (primal)
-  bool svp_reduction(int kappa, int block_size, const b200bkz_param &par)
+  // svp_reduction, bkz.cpp:274-358.  Dual: the block's LAST Gram-Schmidt vector is the one to shorten; the radius is
+  // delta / r(first, first) (exponent negated), while the GH bound and get_pruning still read the primal block.
+  bool svp_reduction(int kappa, int block_size, const b200bkz_param &par, bool dual = false)
   {
-    const int first = kappa;
+    const int first = dual ? kappa + block_size - 1 : kappa;
     size_reduction(0, first + 1, 0);
     double old_first;
     long old_first_expo;
@@ -361,20 +378,28 @@ public:
         st->sec_get += now_s() - tg;
         st->get_calls++;
       }
-      long max_dist_expo = rexpo[0];
-      double max_dist    = rmant[0] * delta();
-      double log_det     = 0;  // get_root_det / get_log_det, gso_interface.cpp:220-242
+      long max_dist_expo = rexpo[first - kappa];
+      double max_dist    = rmant[first - kappa];
+      if (dual)
+      {
+        max_dist      = pow(max_dist, -1.0);  // FP_NR<double>::pow_si(max_dist, -1), nr_FP_d.inl:189-192
+        max_dist_expo = -max_dist_expo;
+      }
+      max_dist *= delta();
+      double log_det = 0;  // get_root_det / get_log_det, gso_interface.cpp:220-242 (the primal block in both cases)
       for (int i = 0; i < block_size; i++)
         log_det += log(ldexp(rmant[i], (int)rexpo[i]));
       const double root_det = exp(log_det / block_size);
       if ((par.flags & B200BKZ_GH_BND) && block_size > 30)
         adjust_radius_to_gh_bound(max_dist, max_dist_expo, block_size, root_det, par.gh_factor);
 
-      // get_pruning, bkz.cpp:82-98 + Strategy::get_pruning, bkz_param.cpp:62-78
+      // get_pruning, bkz.cpp:82-98 + Strategy::get_pruning, bkz_param.cpp:62-78: reads the primal r(kappa, kappa) even
+      // in a dual call, as the reference does
       const Strategy &strat = strategy(block_size);
+      const long kexpo      = rexpo[0];
       double gh_max_dist    = rmant[0];
-      adjust_radius_to_gh_bound(gh_max_dist, max_dist_expo, block_size, root_det, 1.0);
-      const double radius = rmant[0] * pow(2, max_dist_expo), gh = gh_max_dist * pow(2, max_dist_expo);
+      adjust_radius_to_gh_bound(gh_max_dist, kexpo, block_size, root_det, 1.0);
+      const double radius = rmant[0] * pow(2, kexpo), gh = gh_max_dist * pow(2, kexpo);
       const double ghf    = radius / gh;
       const Pruning *pr   = &strat.prune[0];
       double closest      = pow(2, 80);
@@ -385,31 +410,37 @@ public:
           pr      = &p;
         }
 
-      // ExternalEnumeration::enumerate normalisation, enumerate_ext.cpp:64-79,100-106
+      // normalisation as the enumerators do it: primal rdiag scaled by 2^-normexp (enumerate_ext.cpp:64-79,100-106);
+      // a dual radius is a bound on 1/r, so it scales by 2^+normexp (enumerate.cpp:98-105)
       long normexp = -1;
       for (int i = 0; i < block_size; i++)
         normexp = std::max(normexp, rexpo[i] + (long)ilogb(rmant[i]) + 1);
-      const double maxdist_norm = ldexp(max_dist, (int)(max_dist_expo - normexp));
+      const double maxdist_norm = ldexp(max_dist, (int)(dual ? max_dist_expo + normexp : max_dist_expo - normexp));
       for (int i = 0; i < block_size; i++)
         rdiag[i] = ldexp(rmant[i], (int)(rexpo[i] - normexp));
       SolCatch sc;
       sc.d = block_size;
-      b200enum_stats es;
-      std::vector<uint64_t> nodes(block_size);
-      const double t0 = now_s();
-      const int rc    = b200enum_run(block_size, maxdist_norm, mut.data(), rdiag.data(),
-                                     pr->coeff.empty() ? nullptr : pr->coeff.data(), pr->coeff.empty() ? 0 : enum_flags, ctx->devs.data(),
-                                     (int)ctx->devs.size(), 0, 1, sol_cb, &sc, nodes.data(), &es);
-      st->sec_enum += now_s() - t0;
-      st->enum_calls++;
-      if (rc != 0)
-        throw std::runtime_error(std::string("b200enum_run: ") + b200enum_last_error());
-      for (uint64_t v : nodes)
-        st->enum_nodes += v;
+      if (block_size >= 2)
+      {
+        // (a block of one row, the tail of a slide tour, has no vector shorter than delta times its own)
+        b200enum_stats es;
+        std::vector<uint64_t> nodes(block_size);
+        const int eflags = (pr->coeff.empty() ? 0 : enum_flags) | (dual ? B200ENUM_DUAL : 0);
+        const double t0  = now_s();
+        const int rc     = b200enum_run(block_size, maxdist_norm, mut.data(), rdiag.data(),
+                                        pr->coeff.empty() ? nullptr : pr->coeff.data(), eflags, ctx->devs.data(),
+                                        (int)ctx->devs.size(), 0, 1, sol_cb, &sc, nodes.data(), &es);
+        st->sec_enum += now_s() - t0;
+        st->enum_calls++;
+        if (rc != 0)
+          throw std::runtime_error(std::string("b200enum_run: ") + b200enum_last_error());
+        for (uint64_t v : nodes)
+          st->enum_nodes += v;
+      }
 
       if (sc.dist > 0)
       {
-        svp_postprocessing(kappa, block_size, sc.sol);
+        svp_postprocessing(kappa, block_size, sc.sol, dual);
         rerandomize = false;
       }
       else
@@ -421,7 +452,7 @@ public:
     long new_first_expo;
     r_exp(first, new_first, new_first_expo);
     new_first = ldexp(new_first, (int)(new_first_expo - old_first_expo));
-    return old_first <= new_first;
+    return dual ? old_first >= new_first : old_first <= new_first;
   }
 
   // tour / trunc_tour / hkz, bkz.cpp:360-441
@@ -465,6 +496,76 @@ public:
     return clean;
   }
 
+  // trunc_dtour, bkz.cpp:405-417: dual SVP reduction of the blocks ending at max_row - 1, max_row - 2, ..., min_row + block_size
+  bool trunc_dtour(const b200bkz_param &par, int min_row, int max_row)
+  {
+    bool clean = true;
+    for (int kappa = max_row - par.block_size; kappa > min_row; --kappa)
+      clean &= svp_reduction(kappa, par.block_size, par, true);
+    return clean;
+  }
+
+  // sd_tour, bkz.cpp:443-463: a dual tour backwards, then a truncated primal tour forwards
+  bool sd_tour(const b200bkz_param &par, int min_row, int max_row)
+  {
+    int dummy_kappa_max = d;
+    bool clean          = true;
+    clean &= trunc_dtour(par, min_row, max_row);
+    clean &= trunc_tour(dummy_kappa_max, par, min_row, max_row);
+    return clean;
+  }
+
+  // slide_tour, bkz.cpp:465-520: SVP-reduce the disjoint blocks until nothing changes, then dual-SVP-reduce the blocks
+  // shifted by one; progress is measured by the slide potential
+  bool slide_tour(const b200bkz_param &par, int min_row, int max_row)
+  {
+    int p = (max_row - min_row) / par.block_size;
+    if ((max_row - min_row) % par.block_size)
+      ++p;
+    bool clean;  // only for the inner loop
+    do
+    {
+      clean = true;
+      for (int i = 0; i < p; ++i)
+      {
+        const int kappa      = min_row + i * par.block_size;
+        const int block_size = std::min(max_row - kappa, par.block_size);
+        clean &= svp_reduction(kappa, block_size, par);
+      }
+      if (par.flags & B200BKZ_BOUNDED_LLL)  // otherwise svp_preprocessing's LLL from row 0 covers it
+      {
+        long swaps = 0;
+        lll(min_row, min_row, max_row, &swaps);
+        if (swaps > 0)
+          clean = false;
+      }
+    } while (!clean);
+    for (int i = 0; i < p - 1; ++i)
+      svp_reduction(min_row + i * par.block_size + 1, par.block_size, par, true);
+    const double new_potential = slide_potential(min_row, max_row, par.block_size);
+    if (new_potential >= sld_potential)
+      return true;
+    sld_potential = new_potential;
+    return false;
+  }
+
+  // get_slide_potential, gso_interface.cpp:244-258, over get_log_det (:230-242) of the STORED r diagonal (get_r, no
+  // update_gso: the reference reads whatever the last reduction left, and so must the termination test here)
+  double slide_potential(int start_row, int end_row, int block_size)
+  {
+    int p = (end_row - start_row) / block_size;
+    if ((end_row - start_row) % block_size == 0)
+      --p;
+    if (p <= 0)
+      return 0.0;
+    const int n = p * block_size;
+    std::vector<double> mant(n);
+    std::vector<long> expo(n);
+    GCK(b200gso_get_r_diag(g, 0, 0, n, mant.data(), expo.data()));
+    return b200bkz_slide_potential_of(mant.data(), expo.data(), start_row, end_row, block_size);
+  }
+  double sld_potential = 0;
+
   // get_current_slope, gso_interface.cpp:198-218 (requires valid rows: callers run after LLL / a tour)
   double current_slope(int start_row, int stop_row)
   {
@@ -483,15 +584,34 @@ public:
     return v1 / v2;
   }
 
-  // bkz(), bkz.cpp:522-672 (plain BKZ; SD / slide variants are rejected by the caller)
+  // bkz(), bkz.cpp:522-672: plain BKZ, SD-BKZ (B200BKZ_SD_VARIANT) or slide reduction (B200BKZ_SLD_RED)
   int bkz()
   {
-    const int flags  = top.flags;
+    int flags        = top.flags;
     int final_status = 0;
+    const bool sd = (flags & B200BKZ_SD_VARIANT) != 0, sld = (flags & B200BKZ_SLD_RED) != 0;
+    const char *algorithm = sd ? "SD-BKZ" : sld ? "SLD" : "BKZ";
+    if (sd && sld)
+      throw std::runtime_error(B200BKZ_SD_SLD_MSG);
     if (top.block_size < 2)
       return 0;
+    if (sd && !(flags & (B200BKZ_MAX_LOOPS | B200BKZ_MAX_TIME | B200BKZ_AUTO_ABORT)))
+    {
+      fprintf(stderr, "Warning: SD Variant of BKZ requires explicit termination condition. Turning auto abort on!\n");
+      flags |= B200BKZ_AUTO_ABORT;
+    }
+    if (flags & B200BKZ_VERBOSE)
+      fprintf(stderr, "Entering %s: block size %d\n", algorithm, top.block_size);
     GCK(b200gso_discover_all_rows(g));
     const double t_start = now_s();
+    if (sld)
+    {
+      int ok = 1;
+      GCK(b200gso_update_gso(g, &ok));
+      sld_potential = slide_potential(0, d, top.block_size);
+    }
+    if (sd)  // sd-bkz starts with a dual tour, whose size reductions need LLL-reduced lower blocks (bkz.cpp:573-577; the
+      lll(0, 0, d, nullptr, false);  // reference ignores this call's status)
     int no_dec           = -1;
     double old_slope     = std::numeric_limits<double>::max();
     int kappa_max        = -1;
@@ -521,18 +641,38 @@ public:
         if (no_dec >= top.auto_abort_max_no_dec)
           break;
       }
-      clean = tour(i, kappa_max, top, 0, d);
+      if (sd)
+        clean = sd_tour(top, 0, d);
+      else if (sld)
+        clean = slide_tour(top, 0, d);
+      else
+        clean = tour(i, kappa_max, top, 0, d);
       st->tours = i + 1;
       if (flags & B200BKZ_VERBOSE)
       {
         double m;
         long e;
         r_exp(0, m, e);
-        fprintf(stderr, "End of BKZ loop %d, time = %.3fs, r_0 = %.6g, enum nodes = 2^%.2f\n", i, now_s() - t_start,
-                ldexp(m, (int)e), log2((double)st->enum_nodes + 1));
+        fprintf(stderr, "End of %s loop %d, time = %.3fs, r_0 = %.6g, enum nodes = 2^%.2f\n", algorithm, i,
+                now_s() - t_start, ldexp(m, (int)e), log2((double)st->enum_nodes + 1));
       }
       if (clean || top.block_size >= d)
         break;
+    }
+    int dummy_kappa_max = d;
+    if (sd)  // hkz-reduce the last window, which SD-BKZ leaves unreduced (bkz.cpp:626-641)
+      hkz(dummy_kappa_max, top, std::max(d - top.block_size, 0), d);
+    if (sld)
+    {
+      // hkz-reduce the blocks, which slide reduction leaves only SVP- and dual-SVP-reduced (bkz.cpp:642-665)
+      int p = d / top.block_size;
+      if (d % top.block_size)
+        ++p;
+      for (int j = 0; j < p; ++j)
+      {
+        const int kappa = j * top.block_size + 1;
+        hkz(dummy_kappa_max, top, kappa, std::min(d, kappa + top.block_size - 1));
+      }
     }
     return final_status;
   }
@@ -555,6 +695,23 @@ private:
 extern "C" {
 
 const char *b200bkz_last_error(void) { return g_bkz_err.c_str(); }
+
+double b200bkz_slide_potential_of(const double *rmant, const long *rexpo, int start_row, int end_row, int block_size)
+{
+  // get_slide_potential / get_log_det, gso_interface.cpp:230-258, in the reference's order of operations
+  double potential = 0.0;
+  int p            = (end_row - start_row) / block_size;
+  if ((end_row - start_row) % block_size == 0)
+    --p;
+  for (int i = 0; i < p; ++i)
+  {
+    double log_det = 0.0;
+    for (int k = i * block_size; k < (i + 1) * block_size; ++k)
+      log_det += log(ldexp(rmant[k], (int)rexpo[k]));
+    potential += (double)(p - i) * log_det;
+  }
+  return potential;
+}
 
 void b200bkz_default_param(b200bkz_param *p, int block_size)
 {
@@ -611,9 +768,14 @@ int b200bkz_add_strategy(b200bkz_t *h, int block_size, const int *preproc, int n
 
 int b200bkz_reduce(b200bkz_t *h, int d, int n, int64_t *b, const b200bkz_param *param, b200bkz_stats *stats)
 {
-  if (!h || !b || !param || d < 1 || n < 1 || (param->flags & 0x300))
+  if (!h || !b || !param || d < 1 || n < 1)
   {
-    g_bkz_err = "b200bkz_reduce: bad arguments (SD-BKZ / slide reduction are not supported)";
+    g_bkz_err = "b200bkz_reduce: bad arguments";
+    return B200BKZ_EINVAL;
+  }
+  if ((param->flags & B200BKZ_SD_VARIANT) && (param->flags & B200BKZ_SLD_RED))
+  {
+    g_bkz_err = B200BKZ_SD_SLD_MSG;  // bkz.cpp:531-534
     return B200BKZ_EINVAL;
   }
   b200bkz_stats local;

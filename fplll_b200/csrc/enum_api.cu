@@ -29,8 +29,8 @@
 // multiply and subtract (--fmad=false), the order of the reference's center_partsums, so with a fixed radius the set
 // of visited nodes — and therefore the node count — is identical to the reference's own enumerator.
 // Dual enumeration (enumerate_base.cpp:64-68: the chain runs over alpha_j = x_j - c_j instead of x_j, on the reversed
-// inverted basis, enumerate.cpp:100-124) and sub-solutions (enumerate_base.cpp:36-40) are served by the thread-local
-// kernel variant; the tuned shared-memory variant is primal-only.
+// inverted basis, enumerate.cpp:100-124) runs in both kernel variants: the shared-memory one keeps alpha next to x.
+// Sub-solutions (enumerate_base.cpp:36-40) are served by the thread-local variant only.
 #include "../../include/b200enum.h"
 #include <algorithm>
 #include <chrono>
@@ -163,14 +163,16 @@ __device__ inline unsigned long long atomic_add_sys(unsigned long long *p, unsig
 // (a round = every walker works off the current half of the task queue, walkers that split or yield append to the other
 // half).  One launch per Enumeration::enumerate call instead of one launch + host synchronisation per round.
 //
-// XS = true (dim <= 64, every BKZ block size in use; primal, no sub-solutions): the coefficient vectors x[] of all
+// XS = true (dim <= 64, every BKZ block size in use; no sub-solutions): the coefficient vectors x[] of all
 // walkers of the CTA live in SHARED memory ([level][thread], conflict-free) — the centre chain reads x[j] d-k times per
 // node, and with x[] in thread-local memory that traffic (L1 misses for 3/4 of it, ~1.6 KB of L2 reads per node) was
-// what bounded the first version.  One CTA per SM then shares a single copy of mu^T.
+// what bounded the first version.  One CTA per SM then shares a single copy of mu^T.  XDUAL = true is the dual
+// instantiation: the chains read alpha_j, kept in a second [level][thread] array right after x[] (two d-vectors per
+// walker, so the CTA has fewer walkers: launch_shape).  The primal instantiation is compiled without it.
 // Both variants also keep pre[k] = the part of level k's centre chain that only involves the task's FIXED coefficients
 // (j > top0): it is computed the first time the walker reaches level k inside a task and is the exact prefix of the
 // reference's descending chain, so the remaining chain is top0-k long instead of d-1-k.
-template <int ML, bool XS>
+template <int ML, bool XS, bool XDUAL = false>
 __global__ void __launch_bounds__(XS ? THREADS_XS : THREADS) k_enum(EnumArgs a)
 {
   namespace cg = cooperative_groups;
@@ -181,6 +183,7 @@ __global__ void __launch_bounds__(XS ? THREADS_XS : THREADS) k_enum(EnumArgs a)
   double *s_mut = sm, *s_r = sm + (size_t)d * ds, *s_p = s_r + d;
   double *s_x = s_p + d + threadIdx.x;  // XS: x[j] of this thread at s_x[j * blockDim.x]
   const int xstr = blockDim.x;
+  double *s_al = s_x + (size_t)d * xstr;  // XS dual: alpha[j] of this thread at s_al[j * blockDim.x]
   for (int t = threadIdx.x; t < d * d; t += blockDim.x)
     s_mut[(t / d) * ds + (t % d)] = a.mut[t];
   for (int t = threadIdx.x; t < d; t += blockDim.x)
@@ -189,7 +192,7 @@ __global__ void __launch_bounds__(XS ? THREADS_XS : THREADS) k_enum(EnumArgs a)
     s_p[t] = a.prun[t];
   }
   __syncthreads();
-  const bool DUAL = !XS && a.dual, SUBS = !XS && a.findsubsols;
+  const bool DUAL = XS ? XDUAL : (a.dual != 0), SUBS = !XS && a.findsubsols;
 
   double xl[XS ? 1 : ML], al[XS ? 1 : ML], cen[ML], pd[ML], pre[ML];
   unsigned cnt[ML];
@@ -200,8 +203,15 @@ __global__ void __launch_bounds__(XS ? THREADS_XS : THREADS) k_enum(EnumArgs a)
     else
       xl[XS ? 0 : j] = val;
   };
+  auto getal = [&](int j) -> double { return XS ? s_al[(size_t)j * xstr] : al[XS ? 0 : j]; };
+  auto setal = [&](int j, double val) {
+    if (XS)
+      s_al[(size_t)j * xstr] = val;
+    else
+      al[XS ? 0 : j] = val;
+  };
   // what the centre chains multiply mu with: x_j, or alpha_j = x_j - c_j in a dual enumeration
-  auto chainv = [&](int j) -> double { return DUAL ? al[XS ? 0 : j] : getx(j); };
+  auto chainv = [&](int j) -> double { return DUAL ? getal(j) : getx(j); };
   int top0 = 0, pvalid = 0;
 #pragma unroll 1
   for (int k = 0; k < d; k++)
@@ -285,8 +295,8 @@ __global__ void __launch_bounds__(XS ? THREADS_XS : THREADS) k_enum(EnumArgs a)
           const double *mr = s_mut + (size_t)j * ds;
 #pragma unroll 1
           for (int i = d - 1; i > j; --i)
-            c = __dsub_rn(c, __dmul_rn(al[XS ? 0 : i], mr[i]));
-          al[XS ? 0 : j] = __dsub_rn(getx(j), c);
+            c = __dsub_rn(c, __dmul_rn(getal(i), mr[i]));
+          setal(j, __dsub_rn(getx(j), c));
         }
       }
       pd[k]  = h.pd;
@@ -307,7 +317,7 @@ __global__ void __launch_bounds__(XS ? THREADS_XS : THREADS) k_enum(EnumArgs a)
       n++;
       nr++;
       if (DUAL)
-        al[XS ? 0 : k] = alphak;
+        setal(k, alphak);
       if (SUBS && newdist != 0.0 && newdist < __longlong_as_double(*(volatile unsigned long long *)(a.sub_bits + k)))
       {
         // sub-solution (enumerate_base.cpp:36-40): best partial vector per level; the host keeps the per-level minimum
@@ -636,6 +646,7 @@ int get_ctx(int device, DevCtx **out)
   CKE(cudaFuncSetAttribute((const void *)k_enum<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
   CKE(cudaFuncSetAttribute((const void *)k_enum<160, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
   CKE(cudaFuncSetAttribute((const void *)k_enum<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_XS_MAX));
+  CKE(cudaFuncSetAttribute((const void *)k_enum<64, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_XS_MAX));
   g_ctx.push_back(c);
   *out = &g_ctx.back();
   return 0;
@@ -724,22 +735,26 @@ struct LaunchShape
   size_t smem;
 };
 
-int launch_shape(DevCtx *c, int d, bool xs, LaunchShape &ls)
+int launch_shape(DevCtx *c, int d, bool xs, bool dual, LaunchShape &ls)
 {
   const Tuning &tn      = tuning();
   const size_t cfg_n    = (size_t)d * d + 2 * d;
   const size_t cfg_smem = xs ? ((size_t)d * (d | 1) + 2 * d) * sizeof(double) : cfg_n * sizeof(double);
+  // XS: every walker keeps one d-vector in shared memory (x), two in a dual call (x and alpha) — at d = 64 that is 320
+  // walkers per CTA primal (the thread cap) and 192 dual
+  const size_t per_walker = (xs && dual ? 2 : 1) * (size_t)d * sizeof(double);
   int threads = THREADS;
   if (xs)
   {
-    threads = (int)((SMEM_XS_MAX - cfg_smem) / ((size_t)d * sizeof(double)));
+    threads = (int)((SMEM_XS_MAX - cfg_smem) / per_walker);
     threads = std::min(std::min(threads, tn.xs_threads_cap), THREADS_XS) & ~31;
     if (threads < 32)
       threads = 32;
   }
-  ls.smem    = cfg_smem + (xs ? (size_t)threads * d * sizeof(double) : 0);
+  ls.smem    = cfg_smem + (xs ? (size_t)threads * per_walker : 0);
   ls.threads = threads;
-  ls.fn = xs ? (const void *)k_enum<64, true> : (d <= 64 ? (const void *)k_enum<64, false> : (const void *)k_enum<160, false>);
+  ls.fn = xs ? (dual ? (const void *)k_enum<64, true, true> : (const void *)k_enum<64, true>)
+             : (d <= 64 ? (const void *)k_enum<64, false> : (const void *)k_enum<160, false>);
   if (xs)
   {
     ls.blocks = c->sms;  // one CTA per SM by construction (shared memory); every CTA must be resident (grid barrier)
@@ -917,7 +932,7 @@ int run_impl(int dim, double maxdist, const double *mut_in, const double *rdiag_
     }
   }
 
-  const bool xs = tn.use_xs && d <= 64 && !dual && !subs;
+  const bool xs = tn.use_xs && d <= 64 && !subs;  // B200_ENUM_XS=0: the thread-local variant for every call
   auto make_args = [&](DevCtx *c, EnumArgs &a) {
     memset(&a, 0, sizeof(a));
     a.d = d, a.dstride = dstride;
@@ -935,7 +950,7 @@ int run_impl(int dim, double maxdist, const double *mut_in, const double *rdiag_
   };
   auto launch = [&](DevCtx *c, EnumArgs &a) -> int {
     LaunchShape ls;
-    int rc = launch_shape(c, d, xs, ls);
+    int rc = launch_shape(c, d, xs, dual, ls);
     if (rc)
       return rc;
     void *params[] = {(void *)&a};

@@ -30,8 +30,9 @@
 // On top of that, BKZReduction<Z_NR<long>, FP_NR<double>>::bkz() (bkz.cpp:522-672) — what bkz_reduction() / `fplll -a bkz`
 // run after their wrapper-LLL when the basis fits long (bkz.cpp:812-836) — is taken over whole by the device driver
 // (b200bkz_reduce: device-resident LLL loops, device enumeration, no per-call forwarding) whenever the request is one
-// that driver implements (plain BKZ, no transformation matrices, no GSO dump); SD-BKZ / slide reduction keep the
-// reference's control flow over the forwarded GSO.  B200_SHIM_BKZ=0 turns the take-over off.
+// that driver implements: BKZ 2.0, SD-BKZ (-a sdb) and slide reduction (-a sld), without transformation matrices or a GSO
+// dump.  Both SD and slide flags together go to the reference, which throws its own error.  B200_SHIM_BKZ=0 turns the
+// take-over off (every algorithm then runs the reference's control flow over the forwarded GSO).
 //
 // Build (where fplll's headers are installed):  g++ -shared -fPIC fplll_matgso_shim.cpp -lb200bkz -ldl  -> libb200fplll.so
 // Use:  LD_PRELOAD=libb200fplll.so fplll -a bkz -b 40 ...   or link it before -lfplll.   B200_SHIM_STATS=1 prints the
@@ -394,10 +395,13 @@ template <> bool BKZReduction<Z_NR<long>, FP_NR<double>>::bkz()
   static fn_t orig = b200shim::next_symbol<fn_t>("_ZN5fplll12BKZReductionINS_4Z_NRIlEENS_5FP_NRIdEEE3bkzEv");
   static const bool takeover = b200shim::enabled() && !(getenv("B200_SHIM_BKZ") && atoi(getenv("B200_SHIM_BKZ")) == 0);
   auto *mg = dynamic_cast<MatGSO<Z_NR<long>, FP_NR<double>> *>(&m);
-  const int unsupported = BKZ_SD_VARIANT | BKZ_SLD_RED | BKZ_DUMP_GSO;
-  if (!takeover || !mg || (param.flags & unsupported) || mg->enable_int_gram || mg->enable_transform ||
+  const bool sd_and_sld = (param.flags & BKZ_SD_VARIANT) && (param.flags & BKZ_SLD_RED);
+  if (!takeover || !mg || (param.flags & BKZ_DUMP_GSO) || sd_and_sld || mg->enable_int_gram || mg->enable_transform ||
       param.block_size < 2 || num_rows != mg->b.get_rows() || num_rows > 512 || b200gso_device_count() == 0)
     return orig(this);
+  // what the reference's bkz() sets first (bkz.cpp:527-529): set_status prints it under BKZ_VERBOSE, and a null char*
+  // written to cerr would silence the caller's cerr for good
+  algorithm   = (param.flags & BKZ_SD_VARIANT) ? "SD-BKZ" : (param.flags & BKZ_SLD_RED) ? "SLD" : "BKZ";
   const int d = mg->b.get_rows(), n = mg->b.get_cols();
   b200bkz_t *h = nullptr;
   int dev0     = 0;
@@ -423,7 +427,8 @@ template <> bool BKZReduction<Z_NR<long>, FP_NR<double>>::bkz()
   b200bkz_param p;
   b200bkz_default_param(&p, param.block_size);
   p.delta = param.delta, p.flags = (param.flags & (BKZ_VERBOSE | BKZ_MAX_LOOPS | BKZ_MAX_TIME | BKZ_BOUNDED_LLL |
-                                                   BKZ_AUTO_ABORT | BKZ_GH_BND)) | B200BKZ_NO_LLL;
+                                                   BKZ_AUTO_ABORT | BKZ_GH_BND | BKZ_SD_VARIANT | BKZ_SLD_RED)) |
+                                   B200BKZ_NO_LLL;
   p.max_loops = param.max_loops, p.max_time = param.max_time;
   p.auto_abort_scale = param.auto_abort_scale, p.auto_abort_max_no_dec = param.auto_abort_max_no_dec;
   p.gh_factor = param.gh_factor, p.min_success_probability = param.min_success_probability;

@@ -1,7 +1,9 @@
 /* b200bkz.h — C-ABI of the BKZ driver that runs over the device GSO (b200gso.h) and the device enumerator
  * (b200enum.h): the reference's  bkz_reduction(ZZ_mat<long>-regime, FT_DOUBLE)  — fplll/bkz.h:357-426,
- * fplll/bkz.cpp:522-672 (bkz), :274-358 (svp_reduction), :100-126 (svp_preprocessing), :128-272 (svp_postprocessing),
- * :43-80 (rerandomize_block), :360-441 (tour / trunc_tour / hkz), :800-809 (BKZAutoAbort).
+ * fplll/bkz.cpp:522-672 (bkz), :274-358 (svp_reduction, primal and dual), :100-126 (svp_preprocessing), :128-272
+ * (svp_postprocessing), :43-80 (rerandomize_block), :360-441 (tour / trunc_tour / hkz), :405-520 (trunc_dtour / sd_tour /
+ * slide_tour), :800-809 (BKZAutoAbort).  All three algorithms of the reference's bkz(): BKZ 2.0, self-dual BKZ and slide
+ * reduction; only BKZ_DUMP_GSO (0x40) is not supported (B200BKZ_EINVAL).
  *
  * Host C++ keeps only the control flow (which block, which radius, which pruning vector, when to stop); every
  * floating-point GSO update, every LLL / size-reduction call and the enumeration run on the GPU(s).
@@ -16,7 +18,7 @@ extern "C" {
 
 typedef struct b200bkz b200bkz_t;
 
-/* BKZFlags, defs.h:264-274 (SD / slide variants need dual enumeration: not supported, B200BKZ_EINVAL) */
+/* BKZFlags, defs.h:264-274 */
 #define B200BKZ_DEFAULT 0
 #define B200BKZ_VERBOSE 1
 #define B200BKZ_NO_LLL 2
@@ -25,6 +27,10 @@ typedef struct b200bkz b200bkz_t;
 #define B200BKZ_BOUNDED_LLL 0x10
 #define B200BKZ_AUTO_ABORT 0x20
 #define B200BKZ_GH_BND 0x80
+#define B200BKZ_SD_VARIANT 0x100 /* self-dual BKZ: dual tour backwards + primal tour forwards (bkz.cpp:443-463) */
+#define B200BKZ_SLD_RED 0x200    /* slide reduction (bkz.cpp:465-520); exclusive with B200BKZ_SD_VARIANT */
+/* the error both flags together give, word for word the reference's (bkz.cpp:531-534) */
+#define B200BKZ_SD_SLD_MSG "Invalid flags: SD-BKZ and Slide reduction are mutually exclusive!"
 /* Not a reference flag.  By default every PRUNED SVP call enumerates the FIXED region of its initial radius and pruning bounds and
  * takes the shortest vector inside it (ties: smallest coefficient vector): a function of the block alone, so a tour is
  * reproducible run to run and across device counts, and never worse than what the reference's walk returns.  With this
@@ -83,6 +89,9 @@ int b200bkz_add_strategy(b200bkz_t *h, int block_size, const int *preproc, int n
 /* bkz_reduction on a d x n int64 basis, in place.  Returns 0 or a negative error; RedStatus in stats->status. */
 int b200bkz_reduce(b200bkz_t *h, int d, int n, int64_t *b, const b200bkz_param *param, b200bkz_stats *stats);
 const char *b200bkz_last_error(void);
+/* get_slide_potential(start_row, end_row, block_size) (gso_interface.cpp:244-258) of an r diagonal given as mantissa /
+ * exponent pairs (rows 0 .. end_row - 1): what slide reduction's termination test compares tour to tour. */
+double b200bkz_slide_potential_of(const double *rmant, const long *rexpo, int start_row, int end_row, int block_size);
 
 #ifdef __cplusplus
 }
