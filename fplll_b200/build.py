@@ -49,7 +49,7 @@ def build_all(force=False, verbose=False):
     from concurrent.futures import ThreadPoolExecutor
     objdir = os.path.join(LIBDIR, "obj")
     os.makedirs(objdir, exist_ok=True)
-    # B200_NVCC_EXTRA: extra compile flags for experiments, e.g. "-DB200_MU_CACHE=1" (gso_cta.cuh) or -DB200_LLL_PROFILE
+    # B200_NVCC_EXTRA: extra compile flags for experiments, e.g. -DB200_LLL_PROFILE (device-clock phase counters)
     cflags = [f for f in NVCC_FLAGS if f != "-shared"] + os.environ.get("B200_NVCC_EXTRA", "").split()
     units = sorted({u for srcs in TARGETS.values() for u in srcs})
 

@@ -80,11 +80,10 @@ public:
       : ctx(ctx), g(g), d(d), top(top), st(st), rng(top.seed ? top.seed : 0x9e3779b97f4a7c15ull)
   {
     lll_delta = top.delta < 1 ? top.delta : 0.99;  // bkz.cpp:862
-    const char *e = getenv("B200_BKZ_SHRINK");      // experiment knob: 1 forces the shrinking radius, 0 the fixed region
-    const bool shrink = e ? atoi(e) != 0 : (top.flags & B200BKZ_SHRINK_RADIUS) != 0;
-    // (only pruned calls: without pruning the shrinking walk returns the shortest vector of the ball whatever the order,
-    // and the fixed ball would cost an unpruned BKZ-40 tour on dim 180 24 s instead of 1.7 s)
-    enum_flags        = shrink ? 0 : B200ENUM_FIXED_RADIUS;
+    // the fixed region unless the caller asks for the shrinking radius (only pruned calls: without pruning the shrinking
+    // walk returns the shortest vector of the ball whatever the order, and the fixed ball would cost an unpruned BKZ-40
+    // tour on dim 180 24 s instead of 1.7 s)
+    enum_flags = (top.flags & B200BKZ_SHRINK_RADIUS) ? 0 : B200ENUM_FIXED_RADIUS;
   }
   int enum_flags = 0;
 

@@ -107,8 +107,7 @@ __global__ void __launch_bounds__(ST_MAX_CONS * 32, 1)
   stream_update_rows(S, M, i, last_j, ok, smem_st);
 }
 
-template <int MINB>
-__global__ void __launch_bounds__(WARPS_PER_CTA * 32, MINB) k_update_row(Batch S, int i, int last_j, int *ok)
+__global__ void __launch_bounds__(WARPS_PER_CTA * 32, 5) k_update_row(Batch S, int i, int last_j, int *ok)
 {
   View v;
   WarpSmem s;
@@ -378,54 +377,16 @@ __global__ void k_get_block(Batch S, int l, int first, int beta, double *mut, do
 }  // namespace
 
 
-static int upd_variant()
+// ---- tensor maps of the streaming kernel ----
+static bool encode_f64(CUtensorMap *m, void *base, const cuuint64_t *dims, const cuuint64_t *strides,
+                       const cuuint32_t *box, CUtensorMapL2promotion promo)
 {
-  static int v = -1;
-  if (v < 0)
-  {
-    const char *e = getenv("B200_UPD_MINB");  // tuning knob for experiments: CTAs/SM the update kernel is compiled for
-    v             = e ? atoi(e) : 5;
-  }
-  return v;
-}
-// ---- tensor maps of the streaming kernel (driver entry point resolved at run time: no link-time libcuda dependency) ----
-typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
-                                  const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFn encode_tiled_fn()
-{
-  static EncodeTiledFn fn = nullptr;
-  static bool tried       = false;
-  if (!tried)
-  {
-    tried   = true;
-    void *p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
-        q == cudaDriverEntryPointSuccess)
-      fn = (EncodeTiledFn)p;
-  }
-  return fn;
-}
-static bool encode_f64(CUtensorMap *m, void *base, int rank, const cuuint64_t *dims, const cuuint64_t *strides,
-                       const cuuint32_t *box, int l2promo)
-{
-  EncodeTiledFn fn = encode_tiled_fn();
-  if (!fn)
-    return false;
-  const cuuint32_t es[3] = {1, 1, 1};
-  const CUtensorMapL2promotion pr = l2promo == 256   ? CU_TENSOR_MAP_L2_PROMOTION_L2_256B
-                                    : l2promo == 128 ? CU_TENSOR_MAP_L2_PROMOTION_L2_128B
-                                    : l2promo == 64  ? CU_TENSOR_MAP_L2_PROMOTION_L2_64B
-                                                     : CU_TENSOR_MAP_L2_PROMOTION_NONE;
-  return fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT64, (cuuint32_t)rank, base, dims, strides, box, es,
-            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, pr, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+  return tma_encode_f64(m, base, 3, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_NONE, promo);
 }
 // full-panel maps once per handle, the partial-panel maps whenever the row count of the last panel changes
 static bool stream_maps(b200gso *h, int rows_last)
 {
   const Batch &S = h->S;
-  static const int promo = getenv("B200_ST_L2PROMO") ? atoi(getenv("B200_ST_L2PROMO")) : 256;
   const cuuint64_t bf_dims[3] = {32, (cuuint64_t)S.n, (cuuint64_t)S.B * n_panels(S.d)};
   const cuuint64_t bf_str[2]  = {256, (cuuint64_t)256 * S.n};
   const cuuint64_t mu_dims[3] = {32, (cuuint64_t)S.B * (S.mu_stride / 32), 1};
@@ -434,9 +395,9 @@ static bool stream_maps(b200gso *h, int rows_last)
   if (h->st_state == 0)
   {
     const cuuint32_t bx[3] = {32, ST_COLS, 1}, bb[3] = {16, 16, 1};
-    const bool okm = encode_f64(&m[SM_BF_FULL], S.bf, 3, bf_dims, bf_str, bx, promo) &&
-                     encode_f64(&m[SM_MU_FULL], S.mu, 3, mu_dims, mu_str, bx, promo) &&
-                     encode_f64(&m[SM_MU_B], S.mu, 3, mu_dims, mu_str, bb, 128);
+    const bool okm = encode_f64(&m[SM_BF_FULL], S.bf, bf_dims, bf_str, bx, CU_TENSOR_MAP_L2_PROMOTION_L2_256B) &&
+                     encode_f64(&m[SM_MU_FULL], S.mu, mu_dims, mu_str, bx, CU_TENSOR_MAP_L2_PROMOTION_L2_256B) &&
+                     encode_f64(&m[SM_MU_B], S.mu, mu_dims, mu_str, bb, CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
     h->st_state    = okm ? 1 : -1;
     h->st_rows     = 0;
   }
@@ -445,9 +406,12 @@ static bool stream_maps(b200gso *h, int rows_last)
   if (rows_last < 32 && rows_last != h->st_rows)
   {
     const cuuint32_t bx[3] = {(cuuint32_t)rows_last, ST_COLS, 1};
-    const int pp           = rows_last * 8 >= 256 ? 256 : rows_last * 8 >= 128 ? 128 : rows_last * 8 >= 64 ? 64 : 0;
-    if (!encode_f64(&m[SM_BF_PART], S.bf, 3, bf_dims, bf_str, bx, pp) ||
-        !encode_f64(&m[SM_MU_PART], S.mu, 3, mu_dims, mu_str, bx, pp))
+    const CUtensorMapL2promotion pp = rows_last * 8 >= 256   ? CU_TENSOR_MAP_L2_PROMOTION_L2_256B
+                                      : rows_last * 8 >= 128 ? CU_TENSOR_MAP_L2_PROMOTION_L2_128B
+                                      : rows_last * 8 >= 64  ? CU_TENSOR_MAP_L2_PROMOTION_L2_64B
+                                                             : CU_TENSOR_MAP_L2_PROMOTION_NONE;
+    if (!encode_f64(&m[SM_BF_PART], S.bf, bf_dims, bf_str, bx, pp) ||
+        !encode_f64(&m[SM_MU_PART], S.mu, mu_dims, mu_str, bx, pp))
     {
       h->st_state = -1;
       return false;
@@ -475,12 +439,11 @@ static void launch_update_row(b200gso *h, int i, int last_j)
   {
     // consumer warps per CTA: as many as the shared memory holds (<= ST_MAX_CONS), preferring a count that deals the
     // batch evenly over the SMs x NW warps (a warp with one lattice more than the others is the tail of the launch)
-    static const int wmax = getenv("B200_ST_WARPS") ? std::max(1, std::min(ST_MAX_CONS, atoi(getenv("B200_ST_WARPS")))) : ST_MAX_CONS;
     const size_t per = stream_warp_doubles(h->S.d, h->S.n) * sizeof(double);
     const StreamShape sh = stream_shape(i, last_j);
     const int NC         = stream_num_chunks(sh, h->S.n);
     const size_t tabb    = (size_t)NC * sizeof(StreamDesc);
-    const int cap = tabb + per > (size_t)SMEM_OPTIN_MAX ? 0 : (int)std::min<size_t>(wmax, ((size_t)SMEM_OPTIN_MAX - tabb) / per);
+    const int cap = tabb + per > (size_t)SMEM_OPTIN_MAX ? 0 : (int)std::min<size_t>(ST_MAX_CONS, ((size_t)SMEM_OPTIN_MAX - tabb) / per);
     int NW = 0;
     double best = 0;
     for (int w = std::max(1, cap / 2); w <= cap && cap > 0; w++)
@@ -498,12 +461,7 @@ static void launch_update_row(b200gso *h, int i, int last_j)
       return;
     }
   }
-  switch (upd_variant())  // unknown values take <5>, here and in b200gso_resident_lattices
-  {
-  case 8: k_update_row<8><<<g, t, h->smem_compact, h->stream>>>(h->S, i, last_j, h->d_ok); break;
-  case 6: k_update_row<6><<<g, t, h->smem_compact, h->stream>>>(h->S, i, last_j, h->d_ok); break;
-  default: k_update_row<5><<<g, t, h->smem_compact, h->stream>>>(h->S, i, last_j, h->d_ok); break;
-  }
+  k_update_row<<<g, t, h->smem_compact, h->stream>>>(h->S, i, last_j, h->d_ok);
 }
 
 template <class T> static int dev_alloc(b200gso *h, T **p, size_t count)
@@ -549,13 +507,10 @@ int b200gso_create(b200gso_t **out, int batch, int d, int n, int flags, int devi
     return B200GSO_ENODEV;
   }
   CK(cudaSetDevice(device));
-  {
-    // L2 -> DRAM fetch granularity hint.  The panel sweeps issue whole 256-byte lines, but the partial last panel,
-    // the diagonal tiles and the scattered mu(i,.) row write touch single 32-byte sectors; at the default (128 B)
-    // those cost extra DRAM traffic.  B200_L2_FETCH overrides (32/64/128).
-    const char *e = getenv("B200_L2_FETCH");
-    cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, e ? (size_t)atoi(e) : (size_t)32);
-  }
+  // L2 -> DRAM fetch granularity hint.  The panel sweeps issue whole 256-byte lines, but the partial last panel, the
+  // diagonal tiles and the scattered mu(i,.) row write touch single 32-byte sectors; at the default (128 B) those cost
+  // extra DRAM traffic.
+  cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, 32);
   b200gso *h = new b200gso();
   h->device  = device;
   cudaDeviceGetAttribute(&h->sm_count, cudaDevAttrMultiProcessorCount, device);
@@ -621,7 +576,7 @@ int b200gso_create(b200gso_t **out, int batch, int d, int n, int flags, int devi
     b200gso_destroy(h);
     return B200GSO_EINVAL;
   }
-  const void *fns[] = {(const void *)k_init,         (const void *)k_discover_all, (const void *)k_update_row<8>, (const void *)k_update_row<6>, (const void *)k_update_row<5>,
+  const void *fns[] = {(const void *)k_init,         (const void *)k_discover_all, (const void *)k_update_row,
                        (const void *)k_update_row_stream,
                        (const void *)k_update_gso,   (const void *)k_row_addmul_we, (const void *)k_row_op_end,
                        (const void *)k_row_swap,     (const void *)k_move_row,     (const void *)k_upload_row,
@@ -1035,11 +990,9 @@ static int lll_dispatch(b200gso_t *h, int mode, double delta, double eta, int km
   long *d_stats = h->d_stats;
   int *d_st     = (int *)(h->d_stats + 4 * (size_t)S.B + 8);
   // few lattices (BKZ works on one): a whole CTA per lattice (k_lll_cta); many: one warp per lattice, the batch hides
-  // the latencies; the switch-over is two CTAs per SM.  B200_LLL_CTA=0 forces the one-warp kernels, B200_LLL_CTA_MAX moves
-  // the switch-over.
-  const int cta_on  = getenv("B200_LLL_CTA") ? atoi(getenv("B200_LLL_CTA")) : 1;  // read per call: tests switch kernels
-  const int cta_max = getenv("B200_LLL_CTA_MAX") ? atoi(getenv("B200_LLL_CTA_MAX")) : 2 * h->sm_count;
-  const bool cta = cta_on && S.B <= cta_max && S.d > 32;
+  // the latencies; the switch-over is two CTAs per SM.  B200_LLL_CTA=0 forces the one-warp kernels.
+  const int cta_on = getenv("B200_LLL_CTA") ? atoi(getenv("B200_LLL_CTA")) : 1;  // read per call: tests switch kernels
+  const bool cta   = cta_on && S.B <= 2 * h->sm_count && S.d > 32;
   if (cta)
   {
     if (b200gso_lll_cta_launch(h, mode, delta, eta, kmin, kstart, kend, sr_start, d_st, (stats && mode == 0) ? d_stats : nullptr))
@@ -1222,9 +1175,7 @@ int b200gso_resident_lattices(b200gso_t *h)
     return B200GSO_EINVAL;
   cudaSetDevice(h->device);
   int nb = 0, sms = 0;
-  const int v = upd_variant();
-  const void *f = v == 6 ? (const void *)k_update_row<6> : v == 8 ? (const void *)k_update_row<8> : (const void *)k_update_row<5>;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, f, WARPS_PER_CTA * 32, h->smem_compact) != cudaSuccess)
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_update_row, WARPS_PER_CTA * 32, h->smem_compact) != cudaSuccess)
     return B200GSO_ECUDA;
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
   return nb * sms * WARPS_PER_CTA;

@@ -22,19 +22,6 @@
 #pragma once
 #include "gso_warp.cuh"
 
-// Compile-time switches for the shared-memory cache of the leading mu panels (see CoopShared::mu_s; B200_LLL_MU_SMEM=0
-// turns it off at run time) and the CTA-wide move_row (cta_move_row below).  Both validated on hardware in round 2
-// (same LLL / BKZ trajectories; BKZ-60 tour: move_row -1.4 s, mu cache -1.0 s, gpurun_out/r2/bkz60_*.txt).
-#ifndef B200_MU_CACHE
-#define B200_MU_CACHE 1
-#endif
-#ifndef B200_CTA_MOVE
-#define B200_CTA_MOVE 1
-#endif
-#ifndef B200_PUB_SLEEP
-#define B200_PUB_SLEEP 0  // nanoseconds a consumer of a streamed wavefront sleeps between two polls of a slot (0: spin)
-#endif
-
 namespace b200 {
 
 // -DB200_LLL_PROFILE: device-clock counters of the cooperative operations (thread 0 of the one CTA BKZ runs), read back
@@ -87,17 +74,15 @@ struct CoopShared
   View v;      // the master's view (its metadata pointers point into the master's shared-memory cache)
   WarpSmem s;  // the master's scratch rows (vb, rrow, murow, aux, xs)
   double *bm;  // babai_mu row handed to BACKSUB
-#if B200_MU_CACHE
-  // Optional shared-memory cache of the leading mu panels (B200_LLL_MU_SMEM=1; off by default until measured): global
-  // memory stays authoritative — every writer of mu in the LLL path writes through or refreshes the cached copy — and the
-  // readers of the cooperative operations take panels < mu_s_panels from here, so that the kappa-deep serial chains pay
-  // shared-memory instead of L2 latency per tile.
+  // Shared-memory cache of the leading mu panels, as many as fit next to the rest of the CTA's shared memory (none at
+  // large d): global memory stays authoritative — every writer of mu in the LLL path writes through or refreshes the
+  // cached copy — and the readers of the cooperative operations take panels < mu_s_panels from here, so that the
+  // kappa-deep serial chains pay shared-memory instead of L2 latency per tile.
   double *mu_s;
   int mu_s_panels;
   // the last panel of the lattice has only d - 32 (P-1) rows: cached with a column stride just above that (odd), so that
   // at d = 200 (8 rows: stride 9, 16 KB instead of 59 KB) the WHOLE of mu is resident in shared memory
   int mu_last_p, mu_last_stride;
-#endif
   // Streamed wavefronts (the pl - p0 < CTA_WARPS branch of cta_update_gso_row, cta_backsub_stream): pub[2k] = value of
   // column (row) k, pub[2k+1] = its tag (epoch + k), written with ONE 16-byte store so a reader sees both or neither.
   // The owner of a panel publishes every value the moment it is final; the warps of the later panels consume them in
@@ -125,16 +110,10 @@ __device__ inline double pub_wait(const double *slot, double tag)
     asm volatile("ld.volatile.shared.v2.f64 {%0, %1}, [%2];" : "=d"(val), "=d"(t) : "r"(a) : "memory");
     if (t == tag)
       break;
-#if B200_PUB_SLEEP
-    // back off: up to seven warps poll slots of the same panel while its owner's own shared-memory traffic (tile entries,
-    // the published values) has to get through the same load/store queue
-    __nanosleep(B200_PUB_SLEEP);
-#endif
   }
   return val;
 }
 
-#if B200_MU_CACHE
 // The cached copy uses a column stride of 33 doubles instead of the global layout's 32: the forward substitution walks a
 // panel by columns (lanes = 32 rows of one column: consecutive addresses either way), Babai's back-substitution walks it
 // by ROWS (lanes = 32 columns of one row) — with stride 32 that is a 32-way bank conflict on every shared-memory load,
@@ -181,26 +160,6 @@ __device__ inline double coop_mu_load(const CoopShared &C, int i, int k)
 {
   return coop_mu_panel(C, i >> 5)[(size_t)k * coop_mu_stride(C, i >> 5) + (i & 31)];
 }
-#else
-// cache compiled out: the plain global-memory expressions (`v` is the operation's `const View &v = C.v`)
-#define coop_mu_panel(C_, p_) (v.mu + mu_panel_base(p_))
-#define coop_mu_stride(C_, p_) 32
-#define coop_mu_store(C_, i_, k_, val_) (v.mu[mu_off((i_), (k_))] = (val_))
-#define coop_mu_load(C_, i_, k_) (v.mu[mu_off((i_), (k_))])
-struct MuRef
-{
-  const double *mu_g;
-  __device__ inline const double *panel(int p) const { return mu_g + mu_panel_base(p); }
-  __device__ inline int stride(int) const { return 32; }
-  __device__ inline double load(int i, int k) const { return mu_g[mu_off(i, k)]; }
-};
-__device__ inline MuRef mu_ref(const CoopShared &C)
-{
-  MuRef m;
-  m.mu_g = C.v.mu;
-  return m;
-}
-#endif
 
 __device__ inline void cta_bar(int id)
 {
@@ -319,7 +278,7 @@ __device__ inline bool cta_update_diag(CoopShared &C, int i, int last_j, int j0,
 // update_gso_row(i, last_j) for a row that is already discovered and has valid[i] <= last_j (the master checks both).
 // Same arithmetic as warp_update_gso_row: lane l of panel p owns column j = 32p + l,
 //   acc_j = g(i,j); acc_j -= mu(j,k) r(i,k) for k = 0 .. j-1 ascending.
-B200_OPFN bool cta_update_gso_row(CoopShared &C, int i, int last_j, int w, int lane)
+__device__ inline bool cta_update_gso_row(CoopShared &C, int i, int last_j, int w, int lane)
 {
   const View v     = C.v;  // by value: registers, not a reload from shared memory after every store
   const WarpSmem s = C.s;
@@ -556,7 +515,7 @@ B200_OPFN bool cta_update_gso_row(CoopShared &C, int i, int last_j, int w, int l
 // ---- BACKSUB --------------------------------------------------------------------------------------------------------
 // X_j = rnd_we(babai_mu[j]); babai_mu[k] -= X_j * mu(j,k) for k < j, j descending (lll.cpp:202-214).  C.bm holds
 // babai_mu (columns < sr_end); the X_j land in s.xs[j], the per-panel masks of the non-zero ones in xmask[].
-B200_OPFN void cta_backsub(CoopShared &C, int kappa, int sr_end, int sr_start, int w, int lane)
+__device__ inline void cta_backsub(CoopShared &C, int kappa, int sr_end, int sr_start, int w, int lane)
 {
   const View v     = C.v;  // by value: registers, not a reload from shared memory after every store
   const WarpSmem s = C.s;
@@ -734,7 +693,7 @@ B200_OPFN void cta_backsub(CoopShared &C, int kappa, int sr_end, int sr_start, i
 // b_kappa += sum_t lx_t * 2^e_t * b_{row_t} over the nnz compacted rows (lx in s.aux[t], (e << 32 | row) in s.murow[t]):
 // row_addmul_we (gso.cpp:236-262) fused over j; int64 arithmetic wraps, so the order of the additions is immaterial.
 // Warp w takes the column groups w, w + CTA_WARPS, ... of 32 columns.
-B200_OPFN void cta_igemv(CoopShared &C, int kappa, int nnz, int w, int lane)
+__device__ inline void cta_igemv(CoopShared &C, int kappa, int nnz, int w, int lane)
 {
   const View v     = C.v;  // by value: registers, not a reload from shared memory after every store
   const WarpSmem s = C.s;
@@ -780,10 +739,9 @@ B200_OPFN void cta_igemv(CoopShared &C, int kappa, int nnz, int w, int lane)
   CTA_PADD(11, ti0_);
 }
 
-#if B200_MU_CACHE
 // ---- MULOAD --------------------------------------------------------------------------------------------------------
 // (re)fill the shared-memory copies of the mu panels pa..pb (those that are cached) from global memory
-B200_OPFN void cta_mu_load(CoopShared &C, int pa, int pb, int w, int lane)
+__device__ inline void cta_mu_load(CoopShared &C, int pa, int pb, int w, int lane)
 {
   const int tid = threadIdx.x;
   const int hi  = min(pb, C.mu_s_panels - 1);
@@ -818,14 +776,11 @@ B200_OPFN void cta_mu_load(CoopShared &C, int pa, int pb, int w, int lane)
   cta_bar(2);
 }
 
-#endif
-
-#if B200_CTA_MOVE
 // ---- MOVE -----------------------------------------------------------------------------------------------------------
 // move_row(old_r, new_r) (gso.cpp:289-366) by the whole CTA: warp_move_row (gso_warp.cuh) with its lane-strided passes
 // (one column of mu / r / b / bf per lane, one Gram row per lane) strided over all CTA_WARPS * 32 threads instead; the
 // data movement per element is the same, only who carries it differs.
-B200_OPFN void cta_move_row(CoopShared &C, int old_r, int new_r, int w, int lane)
+__device__ inline void cta_move_row(CoopShared &C, int old_r, int new_r, int w, int lane)
 {
   const View v  = C.v;
   const int tid = threadIdx.x, NT = CTA_WARPS * 32;
@@ -905,7 +860,6 @@ B200_OPFN void cta_move_row(CoopShared &C, int old_r, int new_r, int w, int lane
   }
   cta_bar(2);
 }
-#endif
 
 // helper warps: wait for commands until the master says EXIT
 __device__ inline void coop_helper_loop(CoopShared &C, int w, int lane)
@@ -922,14 +876,10 @@ __device__ inline void coop_helper_loop(CoopShared &C, int w, int lane)
       cta_backsub(C, a0, a1, a2, w, lane);
     else if (cmd == COOP_IGEMV)
       cta_igemv(C, a0, a1, w, lane);
-#if B200_MU_CACHE
     else if (cmd == COOP_MULOAD)
       cta_mu_load(C, a0, a1, w, lane);
-#endif
-#if B200_CTA_MOVE
     else if (cmd == COOP_MOVE)
       cta_move_row(C, a0, a1, w, lane);
-#endif
   }
 }
 
@@ -949,23 +899,26 @@ __device__ inline bool lll_update_gso_row(const View &v, int i, int last_j, Warp
     // a single panel: nothing to share.  The one-warp routine writes mu(i, .) to global memory only: refresh the
     // cached copy of that row (mu_off(i, k) = 32 k + i in panel 0)
     const bool ok = warp_update_gso_row(v, i, last_j, s, lane);
-#if B200_MU_CACHE
     if (C->mu_s_panels > 0)
     {
       __syncwarp();
       C->mu_s[coop_mu_stride(*C, 0) * lane + i] = v.mu[32 * lane + i];
       __syncwarp();
     }
-#endif
     return ok;
   }
   coop_post(C, COOP_UPDATE, i, last_j, 0, lane);
   return cta_update_gso_row(*C, i, last_j, 0, lane);
 }
 
+// mu(i,k) as the LLL loop reads it: the one-CTA kernel through its cached panels
+template <bool COOP> __device__ inline double lll_mu_load(const View &v, const CoopShared *C, int i, int k)
+{
+  return COOP ? coop_mu_load(*C, i, k) : v.mu[mu_off(i, k)];
+}
+
 // master: after a one-warp routine rewrote parts of mu in global memory (move_row: rows lo..hi rotate; set_r: the
 // diagonal mirror), bring the cached panels back in line
-#if B200_MU_CACHE
 template <bool COOP> __device__ inline void lll_mu_reload(CoopShared *C, int row_lo, int row_hi, int lane)
 {
   if (!COOP || C->mu_s_panels == 0 || (row_lo >> 5) >= C->mu_s_panels)
@@ -983,9 +936,6 @@ template <bool COOP> __device__ inline void lll_mu_refresh_diag(CoopShared *C, i
   __syncwarp();
 }
 
-#endif
-
-#if B200_CTA_MOVE
 template <bool COOP> __device__ inline void lll_move_row(const View &v, int old_r, int new_r, int lane, CoopShared *C)
 {
   if (!COOP)
@@ -996,6 +946,5 @@ template <bool COOP> __device__ inline void lll_move_row(const View &v, int old_
   coop_post(C, COOP_MOVE, old_r, new_r, 0, lane);
   cta_move_row(*C, old_r, new_r, 0, lane);
 }
-#endif
 
 }  // namespace b200

@@ -10,22 +10,6 @@
 
 namespace b200 {
 
-// mu(i,k) as the LLL code reads it: through the CTA's shared-memory cache when that is compiled in (gso_cta.cuh)
-#if B200_CTA_MOVE
-#define LLL_MOVE_ROW(old_, new_) lll_move_row<COOP>(v, (old_), (new_), lane, C)
-#else
-#define LLL_MOVE_ROW(old_, new_) warp_move_row(v, (old_), (new_), lane)
-#endif
-#if B200_MU_CACHE
-#define LLL_MU_LOAD(i_, k_) (COOP ? coop_mu_load(*C, (i_), (k_)) : v.mu[mu_off((i_), (k_))])
-#define LLL_MU_RELOAD(lo_, hi_) lll_mu_reload<COOP>(C, (lo_), (hi_), lane)
-#define LLL_MU_REFRESH_DIAG(i_) lll_mu_refresh_diag<COOP>(C, (i_), lane)
-#else
-#define LLL_MU_LOAD(i_, k_) (v.mu[mu_off((i_), (k_))])
-#define LLL_MU_RELOAD(lo_, hi_) ((void)0)
-#define LLL_MU_REFRESH_DIAG(i_) ((void)0)
-#endif
-
 enum { RED_SUCCESS = 0, RED_GSO_FAILURE = 2, RED_BABAI_FAILURE = 3, RED_LLL_FAILURE = 4 };  // defs.h:153-169
 constexpr long SIZE_RED_FAILURE_THRESH = 5;                                                    // defs.h:146
 
@@ -54,8 +38,8 @@ struct LLLStats
 // LLLReduction::babai(kappa, size_reduction_end, size_reduction_start), lll.cpp:166-224.
 // MAXQ*32 >= d.  Returns RED_SUCCESS or the failing status (warp-uniform).
 template <int MAXQ, bool COOP = false>
-B200_OPFN int warp_babai(const View &v, WarpSmem &s, int kappa, int sr_end, int sr_start, double eta,
-                                 int lane, long &iters, LLLStats *pst = nullptr, CoopShared *C = nullptr)
+__device__ inline int warp_babai(const View &v, WarpSmem &s, int kappa, int sr_end, int sr_start, double eta, int lane,
+                                 long &iters, LLLStats *pst = nullptr, CoopShared *C = nullptr)
 {
   long max_expo = LONG_MAX;
   for (int iter = 0;; iter++)
@@ -78,7 +62,7 @@ B200_OPFN int warp_babai(const View &v, WarpSmem &s, int kappa, int sr_end, int 
       bm[q]       = 0.0;
       if (k < sr_end)
       {
-        bm[q]          = LLL_MU_LOAD(kappa, k);
+        bm[q]          = lll_mu_load<COOP>(v, C, kappa, k);
         const long de  = v.row_expo_en ? (long)(ek - v.row_expo[k]) : 0;
         s.xs[k]        = 0.0;
         if (k >= sr_start)
@@ -309,7 +293,7 @@ __device__ inline bool warp_b_row_is_zero(const View &v, int i, int lane)
 }
 
 // get_gram(kappa,kappa) (gso.h:314-331) for the Lovasz test; computes the dot product if the entry is invalid.
-B200_OPFN double warp_get_gram_diag(const View &v, WarpSmem &s, int i, int lane)
+__device__ inline double warp_get_gram_diag(const View &v, WarpSmem &s, int i, int lane)
 {
   double *g  = v.gf + tri_off(i) + i;
   double val = *g;
@@ -397,8 +381,8 @@ __device__ inline int warp_lll(const View &v, WarpSmem &s, double *lov, double d
   __syncwarp();
   for (; zeros < d && warp_b_row_is_zero(v, 0, lane); zeros++)
   {
-    LLL_MOVE_ROW(kappa_min, kappa_end - 1 - zeros);
-    LLL_MU_RELOAD(kappa_min, kappa_end - 1 - zeros);
+    lll_move_row<COOP>(v, kappa_min, kappa_end - 1 - zeros, lane, C);
+    lll_mu_reload<COOP>(C, kappa_min, kappa_end - 1 - zeros, lane);
   }
   if (zeros < d)
   {
@@ -454,7 +438,7 @@ __device__ inline int warp_lll(const View &v, WarpSmem &s, double *lov, double d
     // Lovasz test (lll.cpp:110-122): prefix chain lov[i] = lov[i-1] - mu(kappa,i-1) * r(kappa,i-1)
     const double g = warp_get_gram_diag(v, s, kappa, lane);
     for (int k = lane; k < kappa; k += 32)
-      s.aux[k] = __dmul_rn(LLL_MU_LOAD(kappa, k), v.r[tri_off(kappa) + k]);
+      s.aux[k] = __dmul_rn(lll_mu_load<COOP>(v, C, kappa, k), v.r[tri_off(kappa) + k]);
     __syncwarp();
     int new_kappa = kappa, action = 0;  // 0: accept, 1: move_row(old_k,new_kappa), 2: zero vector
     if (lane == 0)
@@ -462,7 +446,7 @@ __device__ inline int warp_lll(const View &v, WarpSmem &s, double *lov, double d
       lov[0] = g;
       (void)serial_chain<true, true>(g, s.aux, kappa, lov);
       // r(k-1,k-1): the diagonal mirror in mu's unused slot (gso_layout.cuh) — shared memory when that panel is cached
-      double thr = __dmul_rn(LLL_MU_LOAD(kappa - 1, kappa - 1), swap_threshold);
+      double thr = __dmul_rn(lll_mu_load<COOP>(v, C, kappa - 1, kappa - 1), swap_threshold);
       if (v.row_expo_en)
         thr = scale2(thr, 2 * (v.row_expo[kappa - 1] - v.row_expo[kappa]));
       if (thr > lov[kappa - 1])
@@ -470,7 +454,7 @@ __device__ inline int warp_lll(const View &v, WarpSmem &s, double *lov, double d
         int kk = kappa;
         for (kk--; kk > kappa_min; kk--)
         {
-          double t2 = __dmul_rn(LLL_MU_LOAD(kk - 1, kk - 1), swap_threshold);
+          double t2 = __dmul_rn(lll_mu_load<COOP>(v, C, kk - 1, kk - 1), swap_threshold);
           if (v.row_expo_en)
             t2 = scale2(t2, 2 * (v.row_expo[kk - 1] - v.row_expo[kappa]));
           if (t2 < lov[kk - 1])
@@ -492,22 +476,22 @@ __device__ inline int warp_lll(const View &v, WarpSmem &s, double *lov, double d
       const int old_k = kappa;
       if (action == 1)
       {
-        LLL_MOVE_ROW(old_k, new_kappa);
-        LLL_MU_RELOAD(new_kappa, old_k);
+        lll_move_row<COOP>(v, old_k, new_kappa, lane, C);
+        lll_mu_reload<COOP>(C, new_kappa, old_k, lane);
         kappa = new_kappa;
       }
       else
       {
         zeros++;
-        LLL_MOVE_ROW(old_k, kappa_end - zeros);
-        LLL_MU_RELOAD(old_k, kappa_end - zeros);
+        lll_move_row<COOP>(v, old_k, kappa_end - zeros, lane, C);
+        lll_mu_reload<COOP>(C, old_k, kappa_end - zeros, lane);
         kappa = old_k;
         continue;
       }
     }
     __syncwarp();
     warp_set_r(v, kappa, kappa, lov[kappa], lane);
-    LLL_MU_REFRESH_DIAG(kappa);
+    lll_mu_refresh_diag<COOP>(C, kappa, lane);
     kappa++;
 #ifdef B200_LLL_PROFILE
     st.cyc_move += clock64() - tm_;

@@ -6,12 +6,7 @@ namespace {
 template <int MAXQ>
 __global__ void __launch_bounds__(CTA_WARPS * 32)
     k_lll_cta(Batch S, int mode, double delta, double eta, int kmin, int kstart, int kend, int sr_start, int *status,
-              long *stats
-#if B200_MU_CACHE
-              ,
-              int mu_panels
-#endif
-    )
+              long *stats, int mu_panels)
 {
   extern __shared__ __align__(16) double smem[];
   const int w = threadIdx.x >> 5, lane = threadIdx.x & 31, l = blockIdx.x;
@@ -38,25 +33,21 @@ __global__ void __launch_bounds__(CTA_WARPS * 32)
     C->bm = bm;
     C->pub = bm + (size_t)((S.d + 32 + 1) & ~1);
     C->epoch = 4096.0;
-#if B200_MU_CACHE
     C->mu_s = bm + 3 * (size_t)((S.d + 32 + 1) & ~1);
     C->mu_s_panels = mu_panels;
     C->mu_last_p = n_panels(S.d) - 1, C->mu_last_stride = mu_s_last_stride(S.d);
-#endif
     C->cmd = COOP_EXIT, C->flag = 1;
   }
   // no slot of the publish array may look like a published value: tags start at 4096
   for (int t = lane; t < 2 * ((S.d + 32 + 1) & ~1); t += 32)
     bm[(size_t)((S.d + 32 + 1) & ~1) + t] = -1.0;
   __syncwarp();
-#if B200_MU_CACHE
   if (mu_panels > 0)
   {
     // shared-memory cache of the leading mu panels: every row the call can touch is < kend
     coop_post(C, COOP_MULOAD, 0, (kend - 1) >> 5, 0, lane);
     cta_mu_load(*C, 0, (kend - 1) >> 5, 0, lane);
   }
-#endif
   LLLStats st;
   st.n_swaps = st.final_kappa = st.zeros = st.babai_iters = 0;
   int r;
@@ -111,36 +102,27 @@ int b200gso_lll_cta_launch(b200gso *h, int mode, double delta, double eta, int k
                            int *d_st, long *d_stats)
 {
   const Batch &S = h->S;
-    size_t sm = cta_smem_doubles(S.d, S.n) * sizeof(double);
-#if B200_MU_CACHE
-#define LLL_CTA_EXTRA_ARG , mu_panels
-    int mu_panels = 0;
-    static const int mu_smem_on = getenv("B200_LLL_MU_SMEM") ? atoi(getenv("B200_LLL_MU_SMEM")) : 1;
-    if (mu_smem_on)
-    {
-      // cache as many leading mu panels as fit into the 227 KB of the CTA
-      // full panels take 32 (p+1) columns of 33 doubles; the last panel of the lattice only its real rows (gso_cta.cuh)
-      const int P = n_panels(S.d);
-      size_t used = 0;
-      while (mu_panels < P)
-      {
-        const size_t cols = 32 * (size_t)(mu_panels + 1);
-        const size_t need = cols * (mu_panels == P - 1 ? mu_s_last_stride(S.d) : MU_SS);
-        if (sm + (used + need) * sizeof(double) > (size_t)227 * 1024)
-          break;
-        used += need;
-        mu_panels++;
-      }
-      sm += used * sizeof(double);
-    }
-#else
-#define LLL_CTA_EXTRA_ARG
-#endif
-    if (S.d <= 128)
-      k_lll_cta<4><<<S.B, CTA_WARPS * 32, sm, h->stream>>>(S, mode, delta, eta, kmin, kstart, kend, sr_start, d_st, d_stats LLL_CTA_EXTRA_ARG);
-    else if (S.d <= 256)
-      k_lll_cta<8><<<S.B, CTA_WARPS * 32, sm, h->stream>>>(S, mode, delta, eta, kmin, kstart, kend, sr_start, d_st, d_stats LLL_CTA_EXTRA_ARG);
-    else
-      k_lll_cta<16><<<S.B, CTA_WARPS * 32, sm, h->stream>>>(S, mode, delta, eta, kmin, kstart, kend, sr_start, d_st, d_stats LLL_CTA_EXTRA_ARG);
+  size_t sm = cta_smem_doubles(S.d, S.n) * sizeof(double);
+  // cache as many leading mu panels as fit into the 227 KB of the CTA
+  // full panels take 32 (p+1) columns of 33 doubles; the last panel of the lattice only its real rows (gso_cta.cuh)
+  const int P   = n_panels(S.d);
+  int mu_panels = 0;
+  size_t used   = 0;
+  while (mu_panels < P)
+  {
+    const size_t cols = 32 * (size_t)(mu_panels + 1);
+    const size_t need = cols * (mu_panels == P - 1 ? mu_s_last_stride(S.d) : MU_SS);
+    if (sm + (used + need) * sizeof(double) > (size_t)227 * 1024)
+      break;
+    used += need;
+    mu_panels++;
+  }
+  sm += used * sizeof(double);
+  if (S.d <= 128)
+    k_lll_cta<4><<<S.B, CTA_WARPS * 32, sm, h->stream>>>(S, mode, delta, eta, kmin, kstart, kend, sr_start, d_st, d_stats, mu_panels);
+  else if (S.d <= 256)
+    k_lll_cta<8><<<S.B, CTA_WARPS * 32, sm, h->stream>>>(S, mode, delta, eta, kmin, kstart, kend, sr_start, d_st, d_stats, mu_panels);
+  else
+    k_lll_cta<16><<<S.B, CTA_WARPS * 32, sm, h->stream>>>(S, mode, delta, eta, kmin, kstart, kend, sr_start, d_st, d_stats, mu_panels);
   return 0;
 }

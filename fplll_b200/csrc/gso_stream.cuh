@@ -26,7 +26,7 @@
 // other state takes warp_update_gso_row (out of line) and the stream skips it.
 #pragma once
 #include "gso_warp.cuh"
-#include <cuda.h>
+#include "tma.cuh"
 
 namespace b200 {
 
@@ -47,67 +47,6 @@ enum { SM_BF_FULL = 0, SM_BF_PART = 1, SM_MU_FULL = 2, SM_MU_PART = 3, SM_MU_B =
 __host__ __device__ inline size_t stream_warp_doubles(int d, int n)
 {
   return ((WarpSmem::doubles(d, n, false) + 15) & ~(size_t)15) + (size_t)ST_STAGES * ST_STAGE_DBL + 16;
-}
-
-__device__ inline unsigned st_smem_u32(const void *p) { return (unsigned)__cvta_generic_to_shared(p); }
-__device__ inline void st_mbar_init(unsigned long long *bar, unsigned count)
-{
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(st_smem_u32(bar)), "r"(count));
-}
-__device__ inline void st_mbar_expect_tx(unsigned long long *bar, unsigned bytes)
-{
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(st_smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ inline void st_mbar_arrive(unsigned long long *bar)
-{
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(st_smem_u32(bar)) : "memory");
-}
-__device__ inline void st_mbar_wait(unsigned long long *bar, unsigned parity)
-{
-  asm volatile("{\n\t"
-               ".reg .pred p;\n\t"
-               "WAIT_%=:\n\t"
-               "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-               "@p bra DONE_%=;\n\t"
-               "bra WAIT_%=;\n\t"
-               "DONE_%=:\n\t"
-               "}" ::"r"(st_smem_u32(bar)),
-               "r"(parity)
-               : "memory");
-}
-__device__ inline bool st_mbar_test(unsigned long long *bar, unsigned parity)
-{
-  unsigned ok;
-  asm volatile("{\n\t"
-               ".reg .pred p;\n\t"
-               "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-               "selp.u32 %0, 1, 0, p;\n\t"
-               "}"
-               : "=r"(ok)
-               : "r"(st_smem_u32(bar)), "r"(parity)
-               : "memory");
-  return ok != 0;
-}
-__device__ inline void st_bulk_1d(void *dst, const void *src, unsigned bytes, unsigned long long *bar)
-{
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                   st_smem_u32(dst)),
-               "l"(src), "r"(bytes), "r"(st_smem_u32(bar))
-               : "memory");
-}
-__device__ inline void st_tensor_2d(void *dst, const CUtensorMap *map, int c0, int c1, unsigned long long *bar)
-{
-  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::
-                   "r"(st_smem_u32(dst)),
-               "l"(map), "r"(c0), "r"(c1), "r"(st_smem_u32(bar))
-               : "memory");
-}
-__device__ inline void st_tensor_3d(void *dst, const CUtensorMap *map, int c0, int c1, int c2, unsigned long long *bar)
-{
-  asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];" ::
-                   "r"(st_smem_u32(dst)),
-               "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(st_smem_u32(bar))
-               : "memory");
 }
 
 // What the row update of ONE lattice looks like to the stream; the same for every streamed lattice of a launch except
@@ -199,16 +138,16 @@ __device__ inline void stream_issue(const Batch &S, const StreamMaps &M, const S
                                     double *dst, unsigned long long *bar)
 {
   const StreamDesc d = tab[e];
-  st_mbar_expect_tx(bar, (unsigned)d.bytes);
+  tma_mbar_expect_tx(bar, (unsigned)d.bytes);
   if (d.map == SM_BROW)
   {
-    st_bulk_1d(dst, S.b + (size_t)l * S.b_stride + (size_t)row_i * S.ldb, (unsigned)d.bytes, bar);
+    tma_bulk_1d(dst, S.b + (size_t)l * S.b_stride + (size_t)row_i * S.ldb, (unsigned)d.bytes, bar);
     return;
   }
   const bool bf = d.map <= SM_BF_PART;
   const int c1  = bf ? d.c1 : d.c1 + l * (int)(S.mu_stride >> 5);
   const int c2  = bf ? d.c2 + l * n_panels(S.d) : 0;
-  st_tensor_3d(dst, &M.m[d.map], bf ? 0 : d.c2, c1, c2, bar);
+  tma_load_3d(dst, &M.m[d.map], bf ? 0 : d.c2, c1, c2, bar);
 }
 
 // ---- consumer ----------------------------------------------------------------------------------------------------------
@@ -228,7 +167,7 @@ struct StreamRing
   int cur_l;     // the lattice being consumed
   bool next_ok;  // the warp's next lattice (cur_l + stride) takes the stream: the table walk may run on into it
   __device__ const double *head() const { return ring + (size_t)(consumed % ST_STAGES) * ST_STAGE_DBL; }
-  __device__ void wait() const { st_mbar_wait(bars + (consumed % ST_STAGES), (consumed / ST_STAGES) & 1u); }
+  __device__ void wait() const { tma_mbar_wait(bars + (consumed % ST_STAGES), (consumed / ST_STAGES) & 1u); }
   __device__ void issue_one(const Batch &S, const StreamMaps &M, int lane)
   {
     if (iss_e == NC)
@@ -507,9 +446,8 @@ __device__ inline void stream_update_rows(const Batch &S, const StreamMaps &M, i
   {
     unsigned long long *bars = (unsigned long long *)(smem_base + (size_t)w * per + (per - 16));
     for (int q = 0; q < ST_STAGES; q++)
-      st_mbar_init(bars + q, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+      tma_mbar_init<1>(bars + q);
+    tma_fence_mbar_init();
   }
   __syncthreads();
   const int l = blockIdx.x * NW + w;

@@ -13,18 +13,6 @@ namespace b200 {
 
 constexpr unsigned FULL = 0xffffffffu;
 
-// The big per-lattice operations.  Inlined into every call site the LLL kernels grow to ~140 k SASS instructions (2.2 MB
-// of code for one resident warp to stream through the instruction caches); -DB200_NOINLINE_OPS=1 keeps one copy of each
-// per kernel.
-#ifndef B200_NOINLINE_OPS
-#define B200_NOINLINE_OPS 0
-#endif
-#if B200_NOINLINE_OPS
-#define B200_OPFN static __device__ __noinline__
-#else
-#define B200_OPFN __device__ inline
-#endif
-
 // per-warp shared-memory scratch (doubles).  full: vb[n] | rrow | murow | aux | xs  (LLL / Babai);
 // compact (update_gso_row only): vb[n] | rrow | murow, aux aliases murow (the diagonal product is formed in place).
 struct WarpSmem
@@ -168,7 +156,7 @@ template <bool SUB, bool PREFIX> __device__ inline double serial_chain(double a,
 }
 
 // MatGSO::update_bf(i), gso.cpp:24-48 for Z_NR<long> (get_f_exp = frexp((double)x), nr_Z_misc.inl:17-22)
-B200_OPFN void warp_update_bf(const View &v, int i, int lane)
+__device__ inline void warp_update_bf(const View &v, int i, int lane)
 {
   const int n = max(v.meta[M_NKC], v.irs[i]);
   const int64_t *brow = v.b + (size_t)i * v.ldb;
@@ -317,7 +305,7 @@ __device__ inline double lane_dot(const double *__restrict__ bfcol /* &bf(j,0) *
 // r(i,k) for k outside the panel comes from shared memory (rrow), inside the panel by shuffle from the lane that
 // has just finished its own chain — the "right-looking" schedule that keeps every chain in reference order.
 // Returns false (warp-uniform) if some mu(i,j) is not finite; gso_valid_cols[i] is then left unchanged.
-B200_OPFN bool warp_update_gso_row(const View &v, int i, int last_j, WarpSmem &s, int lane)
+__device__ inline bool warp_update_gso_row(const View &v, int i, int last_j, WarpSmem &s, int lane)
 {
   if (i >= v.meta[M_NKR])
     warp_discover_row(v, lane);
@@ -444,7 +432,7 @@ B200_OPFN bool warp_update_gso_row(const View &v, int i, int last_j, WarpSmem &s
 }
 
 // row_op_end(first,last), gso_interface.cpp:32-53
-B200_OPFN void warp_row_op_end(const View &v, int first, int last, int lane)
+__device__ inline void warp_row_op_end(const View &v, int first, int last, int lane)
 {
   const int nkr = v.meta[M_NKR];
   for (int i = first; i < last; i++)
@@ -563,7 +551,7 @@ template <class T, class At> __device__ inline void rotate_seq(At at, int lo, in
 // gso_valid_cols are done column-by-column (each lane carries one column through the rotated rows, no scratch);
 // only the entries that can still be valid after the call (columns < min(old,new), SURVEY Appendix A) are moved
 // for mu and r.  The symmetric row+column rotation of gf (matrix.cpp:65-93) goes through v.scratch.
-B200_OPFN void warp_move_row(const View &v, int old_r, int new_r, int lane)
+__device__ inline void warp_move_row(const View &v, int old_r, int new_r, int lane)
 {
   if (old_r == new_r)
     return;

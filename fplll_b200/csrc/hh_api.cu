@@ -9,10 +9,10 @@
 // In a batch the serial chain of one warp hides behind the other resident warps' HBM streaming (update_R moves
 // 16*T(i) bytes per lattice, 1.3 MB at i = 399, n = 400).
 #include "../../include/b200hh.h"
+#include "tma.cuh"
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
-#include <cuda.h>
 #include <cuda_runtime.h>
 #include <algorithm>
 #include <math_constants.h>
@@ -746,41 +746,6 @@ struct XMaps
   CUtensorMap V, R;  // {d*n, B}, box {16, 32}, SWIZZLE_128B
 };
 
-__device__ inline unsigned x_smem_u32(const void *p) { return (unsigned)__cvta_generic_to_shared(p); }
-__device__ inline void x_mbar_wait(unsigned long long *bar, unsigned parity)
-{
-  asm volatile("{\n\t"
-               ".reg .pred p;\n\t"
-               "XW_%=:\n\t"
-               "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-               "@p bra XD_%=;\n\t"
-               "bra XW_%=;\n\t"
-               "XD_%=:\n\t"
-               "}" ::"r"(x_smem_u32(bar)),
-               "r"(parity)
-               : "memory");
-}
-__device__ inline bool x_mbar_test(unsigned long long *bar, unsigned parity)
-{
-  unsigned ok;
-  asm volatile("{\n\t"
-               ".reg .pred p;\n\t"
-               "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-               "selp.u32 %0, 1, 0, p;\n\t"
-               "}"
-               : "=r"(ok)
-               : "r"(x_smem_u32(bar)), "r"(parity)
-               : "memory");
-  return ok != 0;
-}
-__device__ inline void x_tma_2d(void *dst, const CUtensorMap *map, int c0, int c1, unsigned long long *bar)
-{
-  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::
-                   "r"(x_smem_u32(dst)),
-               "l"(map), "r"(c0), "r"(c1), "r"(x_smem_u32(bar))
-               : "memory");
-}
-
 // lane r's 16 elements of a swizzled box: element k at row r, 16-byte column (k >> 1) ^ (r & 7).  (Dense 256-byte rows
 // read back with a per-lane skew were tried too — half the TMA row requests — and were slower.)
 __device__ inline void x_read_box(const double *box, int lane, double (&v)[X_K])
@@ -826,18 +791,13 @@ struct XmCtl
 };
 __device__ inline void xm_store_release(int *p, int v)
 {
-  asm volatile("st.release.cta.shared.s32 [%0], %1;" ::"r"(x_smem_u32(p)), "r"(v) : "memory");
+  asm volatile("st.release.cta.shared.s32 [%0], %1;" ::"r"(tma_smem_u32(p)), "r"(v) : "memory");
 }
 __device__ inline int xm_load_acquire(const int *p)
 {
   int v;
-  asm volatile("ld.acquire.cta.shared.s32 %0, [%1];" : "=r"(v) : "r"(x_smem_u32(p)) : "memory");
+  asm volatile("ld.acquire.cta.shared.s32 %0, [%1];" : "=r"(v) : "r"(tma_smem_u32(p)) : "memory");
   return v;
-}
-
-__device__ inline void xm_arrive(unsigned long long *bar)
-{
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(x_smem_u32(bar)) : "memory");
 }
 
 // chunk sequence in pass-major order: pass q = 0 loads R_i (k0 = 0, 16, ...); pass q >= 1 is reflection j = q - 2 (j = -1:
@@ -883,17 +843,16 @@ __global__ void __launch_bounds__(XM_WARPS * 32, 1) hk_update_R_x32(HBatch S, in
   {
     for (int q = 0; q < XM_S; q++)
     {
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(x_smem_u32(&C->full[q])));
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(x_smem_u32(&C->empty[q])));
+      tma_mbar_init<1>(&C->full[q]);
+      tma_mbar_init<1>(&C->empty[q]);
     }
     for (int q = 0; q < XM_PR; q++)
     {
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(x_smem_u32(&C->pready[q])));
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(x_smem_u32(&C->pfree[q])));
+      tma_mbar_init<1>(&C->pready[q]);
+      tma_mbar_init<1>(&C->pfree[q]);
     }
     C->pass_done = 0;
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    tma_fence_mbar_init();
   }
   __syncthreads();
 
@@ -912,26 +871,24 @@ __global__ void __launch_bounds__(XM_WARPS * 32, 1) hk_update_R_x32(HBatch S, in
       bool active = !it.done(i);
       while (__any_sync((1u << XM_S) - 1u, active))
       {
-        if (active && x_mbar_test(&C->empty[lane], ((g / XM_S) & 1u) ^ 1u))
+        if (active && tma_mbar_test(&C->empty[lane], ((g / XM_S) & 1u) ^ 1u))
         {
           double *dst             = ring + (size_t)lane * X_STAGE_DBL;
           unsigned long long *bar = &C->full[lane];
           const int j             = it.q - 2;
           if (it.q == 0)
           {
-            asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(x_smem_u32(bar)), "r"(X_HALF_DBL * 8) : "memory");
-            x_tma_2d(dst, &M.R, i * n + it.k0, l0, bar);
+            tma_mbar_expect_tx(bar, X_HALF_DBL * 8);
+            tma_load_2d(dst, &M.R, i * n + it.k0, l0, bar);
           }
           else
           {
             const bool hasA = j >= 0, hasB = j + 1 < i;
-            asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(x_smem_u32(bar)),
-                         "r"((int)(hasA + hasB) * X_HALF_DBL * 8)
-                         : "memory");
+            tma_mbar_expect_tx(bar, (int)(hasA + hasB) * X_HALF_DBL * 8);
             if (hasA)
-              x_tma_2d(dst, &M.V, j * n + it.k0, l0, bar);
+              tma_load_2d(dst, &M.V, j * n + it.k0, l0, bar);
             if (hasB)
-              x_tma_2d(dst + X_HALF_DBL, &M.V, (j + 1) * n + it.k0, l0, bar);
+              tma_load_2d(dst + X_HALF_DBL, &M.V, (j + 1) * n + it.k0, l0, bar);
           }
           for (int q = 0; q < XM_S && !it.done(i); q++)
             it.next(n);
@@ -968,8 +925,8 @@ __global__ void __launch_bounds__(XM_WARPS * 32, 1) hk_update_R_x32(HBatch S, in
       }
       // the product slot first: the chain warp consumes in order, so "slot g % 8 is free" also means chunk g - 8 — the
       // previous user of this TMA stage — has landed and been consumed, and the parity wait below cannot see a stale phase
-      x_mbar_wait(&C->pfree[g % XM_PR], ((g / XM_PR) & 1u) ^ 1u);
-      x_mbar_wait(&C->full[g % XM_S], (g / XM_S) & 1u);
+      tma_mbar_wait(&C->pfree[g % XM_PR], ((g / XM_PR) & 1u) ^ 1u);
+      tma_mbar_wait(&C->full[g % XM_S], (g / XM_S) & 1u);
       const double *st = ring + (size_t)(g % XM_S) * X_STAGE_DBL;
       double *rp = Rk + (size_t)k0 * 32 + lane;
       if (q == 0)
@@ -1025,8 +982,8 @@ __global__ void __launch_bounds__(XM_WARPS * 32, 1) hk_update_R_x32(HBatch S, in
       __syncwarp();
       if (lane == 0)
       {
-        xm_arrive(&C->pready[g % XM_PR]);
-        xm_arrive(&C->empty[g % XM_S]);
+        tma_mbar_arrive(&C->pready[g % XM_PR]);
+        tma_mbar_arrive(&C->empty[g % XM_S]);
       }
     }
   }
@@ -1039,7 +996,7 @@ __global__ void __launch_bounds__(XM_WARPS * 32, 1) hk_update_R_x32(HBatch S, in
     for (unsigned g = 0; !it.done(i); g++, it.next(n))
     {
       const int q = it.q, j = q - 2, k0 = it.k0;
-      x_mbar_wait(&C->pready[g % XM_PR], (g / XM_PR) & 1u);
+      tma_mbar_wait(&C->pready[g % XM_PR], (g / XM_PR) & 1u);
       if (q >= 1 && j + 1 < i)
       {
         const double *ps = prod + (size_t)(g % XM_PR) * X_HALF_DBL + lane;
@@ -1066,7 +1023,7 @@ __global__ void __launch_bounds__(XM_WARPS * 32, 1) hk_update_R_x32(HBatch S, in
       }
       __syncwarp();
       if (lane == 0)
-        xm_arrive(&C->pfree[g % XM_PR]);
+        tma_mbar_arrive(&C->pfree[g % XM_PR]);
       if (it.last_of_pass(n))
       {
         // pass q is closed: f of reflection j + 1 (the factor of pass q + 1) is minus the dot product just accumulated
@@ -1126,29 +1083,21 @@ template <class T> static int hh_alloc(b200hh *h, T **p, size_t count)
 }
 static int hgrid(const b200hh *h) { return (h->S.B + HW - 1) / HW; }
 
-// tensor maps of the lane-per-lattice kernel (driver entry point resolved at run time: no link-time libcuda dependency)
+// tensor maps of the lane-per-lattice kernel
 static bool x_maps(b200hh *h)
 {
   if (h->x_state)
     return h->x_state > 0;
   h->x_state = -1;
-  typedef CUresult (*EncodeFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
-                               const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle,
-                               CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-  void *p = nullptr;
-  cudaDriverEntryPointQueryResult q;
-  if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess)
-    return false;
   const HBatch &S = h->S;
   const size_t dn = (size_t)S.d * S.n;
   if (dn % 2)
     return false;  // lattice stride must be a multiple of 16 bytes
   const cuuint64_t dims[2] = {(cuuint64_t)dn, (cuuint64_t)S.B}, str[1] = {(cuuint64_t)dn * 8};
-  const cuuint32_t box[2] = {X_K, 32}, es[2] = {1, 1};
+  const cuuint32_t box[2] = {X_K, 32};
   for (int w = 0; w < 2; w++)
-    if (((EncodeFn)p)(w ? &h->xmaps.R : &h->xmaps.V, CU_TENSOR_MAP_DATA_TYPE_FLOAT64, 2, w ? (void *)S.R : (void *)S.V, dims, str,
-                      box, es, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
+    if (!tma_encode_f64(w ? &h->xmaps.R : &h->xmaps.V, w ? (void *)S.R : (void *)S.V, 2, dims, str, box,
+                        CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B))
       return false;
   h->x_state = 1;
   return true;

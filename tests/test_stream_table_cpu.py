@@ -21,7 +21,7 @@ def exe():
     if not shutil.which("nvcc"):
         pytest.skip("nvcc not available")
     os.makedirs(os.path.dirname(EXE), exist_ok=True)
-    deps = [SRC] + [os.path.join(ROOT, "fplll_b200", "csrc", f) for f in ("gso_stream.cuh", "gso_warp.cuh", "gso_layout.cuh")]
+    deps = [SRC] + [os.path.join(ROOT, "fplll_b200", "csrc", f) for f in ("gso_stream.cuh", "tma.cuh", "gso_warp.cuh", "gso_layout.cuh")]
     if not os.path.exists(EXE) or any(os.path.getmtime(p) > os.path.getmtime(EXE) for p in deps):
         subprocess.check_call(["nvcc", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-o", EXE, SRC])
     return EXE
