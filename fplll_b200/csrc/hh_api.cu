@@ -433,6 +433,9 @@ template <int NPL> __global__ void hk_update_R(HBatch S, int i, int last_j)
     w_update_R<NPL>(v, i, last_j, sR, sP, lane);
 }
 
+// the widest NPL instantiation bounds the row width update_R and hlll accept
+static_assert((B200HH_MAX_N + 31) / 32 + 1 <= 32, "B200HH_MAX_N needs more than 32 elements per lane");
+
 static void launch_update_R(const HBatch &S, int grid, size_t smem, cudaStream_t st, int i, int last_j)
 {
   // a lane's slice of a row must fit NPL registers even when the row starts in the middle of a 32-column group
@@ -1252,9 +1255,18 @@ int b200hh_refresh_R(b200hh_t *h, int i)
 {
   HH_CALL(i >= 0 && i < h->S.d, (hk_refresh_R<<<hgrid(h), HW * 32, h->smem, h->stream>>>(h->S, i)))
 }
+// update_R and hlll keep a lane's share of a reflection in registers: rows wider than B200HH_MAX_N do not fit
+static bool width_ok(const b200hh *h, const char *fn)
+{
+  if (h->S.n <= B200HH_MAX_N)
+    return true;
+  g_err = std::string(fn) + ": n = " + std::to_string(h->S.n) + " exceeds B200HH_MAX_N = " + std::to_string(B200HH_MAX_N);
+  return false;
+}
+
 int b200hh_update_R(b200hh_t *h, int i, int last_j)
 {
-  HH_CALL(i >= 0 && i < h->S.d && h->S.n <= 32 * 31, launch_update_R_h(h, i, last_j))
+  HH_CALL(i >= 0 && i < h->S.d && width_ok(h, "b200hh_update_R"), launch_update_R_h(h, i, last_j))
 }
 int b200hh_update_R_last(b200hh_t *h, int i)
 {
@@ -1333,7 +1345,7 @@ int b200hh_get_state(b200hh_t *h, double *R, double *V, double *bf, double *sigm
 
 int b200hh_time_update_R(b200hh_t *h, int i, int reps, float *ms_update_mean)
 {
-  if (!h || !ms_update_mean || reps <= 0 || i < 0 || i >= h->S.d)
+  if (!h || !ms_update_mean || reps <= 0 || i < 0 || i >= h->S.d || !width_ok(h, "b200hh_time_update_R"))
     return B200HH_EINVAL;
   CKH(cudaSetDevice(h->device));
   std::vector<cudaEvent_t> ev(2 * (size_t)reps);
@@ -1372,6 +1384,8 @@ int b200hh_hlll(b200hh_t *h, double delta, double eta, double theta, double c, i
     g_err = "b200hh_hlll: the handle was created without keep_history (recover_R needs R_history)";
     return B200HH_EINVAL;
   }
+  if (!width_ok(h, "b200hh_hlll"))
+    return B200HH_EINVAL;
   CKH(cudaSetDevice(h->device));
   const HBatch &S = h->S;
   const size_t bd = (size_t)S.B * S.d;

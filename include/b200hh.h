@@ -28,6 +28,11 @@ typedef struct b200hh b200hh_t;
 #define B200HH_ECUDA (-3)
 #define B200HH_ENOMEM (-4)
 
+/* Widest row update_R and hlll accept: a lane keeps its share of a reflection (ceil(n/32) + 1 elements, the row may
+ * start inside a 32-column group) in at most 32 registers.  Wider handles can be created and use the other entry
+ * points; b200hh_update_R, b200hh_time_update_R and b200hh_hlll return B200HH_EINVAL for them. */
+#define B200HH_MAX_N (32 * 31)
+
 const char *b200hh_last_error(void);
 
 /* MatHouseholder ctor, householder.h:41-135.  b: batch*d*n int64 row-major.  keep_history != 0 allocates the

@@ -367,8 +367,52 @@ def live_fixtures():
     json.dump(excerpt, open(os.path.join(HERE, "strategies_default_excerpt.json"), "w"), separators=(",", ":"))
 
 
+def size_class_inputs():
+    """Seeded inputs of size_classes_ref.npz, which stores them for the tests: device LLL above 256 rows (d = 300, 12-bit entries;
+    a d = 260 knapsack whose 40-60-bit column makes Babai round large X) and device HLLL with rows wider than 416
+    columns (d = 30, n = 600)."""
+    rng = np.random.default_rng(300)
+    lll300 = rng.integers(-(1 << 12), 1 << 12, size=(300, 301), dtype=np.int64)
+    knap260 = np.zeros((260, 261), np.int64)
+    knap260[:, 0] = rng.integers(1 << 40, 1 << 60, size=260)
+    knap260[np.arange(260), np.arange(260) + 1] = 1
+    # 30 random rows of 600 columns are nearly orthogonal already: mix them so that HLLL has to work
+    hlll600 = rng.integers(-64, 65, size=(30, 30)) @ rng.integers(-(1 << 10), 1 << 10, size=(30, 600))
+    return dict(lll300=lll300, knap260=knap260, hlll600=hlll600)
+
+
+def _narrow(a):
+    """the smallest integer type that holds a exactly (keeps the fixture small; readers widen to int64)."""
+    for t in (np.int16, np.int32):
+        if np.abs(a).max() <= np.iinfo(t).max:
+            return a.astype(t)
+    return a
+
+
+def size_class_fixtures():
+    """tests/golden/size_classes_ref.npz (python tests/golden/make_golden.py --sizes, a few seconds): the reference's
+    LLLReduction over MatGSO<long,double> with GSO_ROW_EXPO (ref_probe lll_long) and HLLLReduction<long,double>
+    (hlll_long) on size_class_inputs(): input, output basis, status and, for LLL, the swap count."""
+    pack = {}
+    for tag, b in size_class_inputs().items():
+        inp, outp = os.path.join(TMP, "size_%s_in.txt" % tag), os.path.join(TMP, "size_%s_out.txt" % tag)
+        O.write_matrix(inp, b)
+        cmd = "hlll_long 0.99 0.51 0.001 0.1" if tag.startswith("hlll") else "lll_long 0.99 0.51"
+        o = O.run_ref("load %s\ntolong\n%s\nsave_long %s\n" % (inp, cmd, outp), timeout=600)
+        tok = dict(t.split("=") for t in o.split(cmd.split()[0] + " ")[1].split() if "=" in t)
+        pack[tag + "_in"] = _narrow(b)
+        pack[tag + "_out"] = _narrow(np.array(O.read_matrix(outp), dtype=np.int64))
+        pack[tag + "_status"] = np.int32(tok["status"])
+        if "swaps" in tok:
+            pack[tag + "_swaps"] = np.int32(tok["swaps"])
+        print(tag, o.strip(), flush=True)
+    np.savez_compressed(os.path.join(HERE, "size_classes_ref.npz"), **pack)
+
+
 if __name__ == "__main__":
-    if "--live" in sys.argv:
+    if "--sizes" in sys.argv:
+        size_class_fixtures()
+    elif "--live" in sys.argv:
         live_fixtures()
     elif "--config2" in sys.argv:
         config2_mpz_reference()

@@ -87,6 +87,15 @@ def test_oracle_hlll_equals_reference_golden(tag):
     assert np.array_equal(m.state()["b"], g[tag + "_out"])
 
 
+def test_oracle_hlll_n600_matches_reference():
+    """rows of 600 columns: the reference's HLLLReduction<long,double> result is in tests/golden/size_classes_ref.npz
+    (make_golden.py --sizes)."""
+    z = H.gold("size_classes_ref.npz")
+    m = O.OracleHouseholder(z["hlll600_in"].astype(np.int64))
+    assert m.hlll(0.99, 0.51, 0.001, 0.1) == int(z["hlll600_status"]) == 0
+    assert np.array_equal(m.state()["b"], z["hlll600_out"])
+
+
 HLLL_LIVE_CASES = [(5, 30, 25), (6, 50, 12), (7, 70, 40)]
 
 

@@ -58,6 +58,18 @@ def test_lll_u40_matches_reference_basis():
     assert np.array_equal(m.state()["b"], z["b_out"])
 
 
+@pytest.mark.parametrize("tag", ["lll300", "knap260"])
+def test_lll_above_256_rows_matches_reference_basis(tag):
+    """d = 300 uniform and a d = 260 knapsack: the reference's LLLReduction<long,double> results are in
+    tests/golden/size_classes_ref.npz (make_golden.py --sizes)."""
+    z = H.gold("size_classes_ref.npz")
+    m = O.OracleGSO(z[tag + "_in"].astype(np.int64))
+    res = m.lll(0.99, 0.51)
+    assert res["status"] == int(z[tag + "_status"]) == 0
+    assert res["n_swaps"] == int(z[tag + "_swaps"])
+    assert np.array_equal(m.state()["b"], z[tag + "_out"])
+
+
 GSO_OPS_CASES = [(1, 12, 12, 20), (2, 33, 40, 30), (3, 64, 65, 12), (4, 7, 9, 50)]
 
 
