@@ -6,7 +6,6 @@
 // sweep loops) is what hides DRAM latency, not shared-memory tiling.  There is no CPU fallback anywhere.
 #include "gso_common.cuh"
 #include "gso_gram.cuh"
-#include "gso_stream.cuh"
 
 thread_local std::string b200gso_g_err;
 long b200gso_g_prof[8] = {0, 0, 0, 0, 0, 0, 0, 0};
@@ -97,14 +96,6 @@ __global__ void k_discover_all(Batch S, int upto)
     return;
   while (v.meta[M_NKR] < upto)
     warp_discover_row(v, lane);
-}
-
-// TMA-fed streaming variant (gso_stream.cuh): one persistent CTA per SM, every warp walks its own lattices
-__global__ void __launch_bounds__(ST_MAX_CONS * 32, 1)
-    k_update_row_stream(const __grid_constant__ Batch S, int i, int last_j, int *ok, const __grid_constant__ StreamMaps M)
-{
-  extern __shared__ __align__(128) double smem_st[];
-  stream_update_rows(S, M, i, last_j, ok, smem_st);
 }
 
 __global__ void __launch_bounds__(WARPS_PER_CTA * 32, 5) k_update_row(Batch S, int i, int last_j, int *ok)
@@ -376,92 +367,9 @@ __global__ void k_get_block(Batch S, int l, int first, int beta, double *mut, do
 
 }  // namespace
 
-
-// ---- tensor maps of the streaming kernel ----
-static bool encode_f64(CUtensorMap *m, void *base, const cuuint64_t *dims, const cuuint64_t *strides,
-                       const cuuint32_t *box, CUtensorMapL2promotion promo)
-{
-  return tma_encode_f64(m, base, 3, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_NONE, promo);
-}
-// full-panel maps once per handle, the partial-panel maps whenever the row count of the last panel changes
-static bool stream_maps(b200gso *h, int rows_last)
-{
-  const Batch &S = h->S;
-  const cuuint64_t bf_dims[3] = {32, (cuuint64_t)S.n, (cuuint64_t)S.B * n_panels(S.d)};
-  const cuuint64_t bf_str[2]  = {256, (cuuint64_t)256 * S.n};
-  const cuuint64_t mu_dims[3] = {32, (cuuint64_t)S.B * (S.mu_stride / 32), 1};
-  const cuuint64_t mu_str[2]  = {256, (cuuint64_t)256 * S.B * (S.mu_stride / 32)};
-  CUtensorMap *m = h->st_maps.m;
-  if (h->st_state == 0)
-  {
-    const cuuint32_t bx[3] = {32, ST_COLS, 1}, bb[3] = {16, 16, 1};
-    const bool okm = encode_f64(&m[SM_BF_FULL], S.bf, bf_dims, bf_str, bx, CU_TENSOR_MAP_L2_PROMOTION_L2_256B) &&
-                     encode_f64(&m[SM_MU_FULL], S.mu, mu_dims, mu_str, bx, CU_TENSOR_MAP_L2_PROMOTION_L2_256B) &&
-                     encode_f64(&m[SM_MU_B], S.mu, mu_dims, mu_str, bb, CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
-    h->st_state    = okm ? 1 : -1;
-    h->st_rows     = 0;
-  }
-  if (h->st_state < 0)
-    return false;
-  if (rows_last < 32 && rows_last != h->st_rows)
-  {
-    const cuuint32_t bx[3] = {(cuuint32_t)rows_last, ST_COLS, 1};
-    const CUtensorMapL2promotion pp = rows_last * 8 >= 256   ? CU_TENSOR_MAP_L2_PROMOTION_L2_256B
-                                      : rows_last * 8 >= 128 ? CU_TENSOR_MAP_L2_PROMOTION_L2_128B
-                                      : rows_last * 8 >= 64  ? CU_TENSOR_MAP_L2_PROMOTION_L2_64B
-                                                             : CU_TENSOR_MAP_L2_PROMOTION_NONE;
-    if (!encode_f64(&m[SM_BF_PART], S.bf, bf_dims, bf_str, bx, pp) ||
-        !encode_f64(&m[SM_MU_PART], S.mu, mu_dims, mu_str, bx, pp))
-    {
-      h->st_state = -1;
-      return false;
-    }
-    h->st_rows = rows_last;
-  }
-  else if (h->st_rows == 0)
-  {
-    // never used by a launch without a partial panel, but the parameter block must hold valid descriptors
-    m[SM_BF_PART] = m[SM_BF_FULL];
-    m[SM_MU_PART] = m[SM_MU_FULL];
-    h->st_rows    = 32;
-  }
-  return true;
-}
-
 static void launch_update_row(b200gso *h, int i, int last_j)
 {
-  const int g = grid_warps(h), t = WARPS_PER_CTA * 32;
-  // B200_UPD_STREAM=0: the register-staged kernel (k_update_row) for every launch
-  // (read per call: the parity tests switch kernels inside one process)
-  const char *us_      = getenv("B200_UPD_STREAM");
-  const int use_stream = us_ ? atoi(us_) : 0;
-  if (use_stream && !h->S.host_basis)
-  {
-    // consumer warps per CTA: as many as the shared memory holds (<= ST_MAX_CONS), preferring a count that deals the
-    // batch evenly over the SMs x NW warps (a warp with one lattice more than the others is the tail of the launch)
-    const size_t per = stream_warp_doubles(h->S.d, h->S.n) * sizeof(double);
-    const StreamShape sh = stream_shape(i, last_j);
-    const int NC         = stream_num_chunks(sh, h->S.n);
-    const size_t tabb    = (size_t)NC * sizeof(StreamDesc);
-    const int cap = tabb + per > (size_t)SMEM_OPTIN_MAX ? 0 : (int)std::min<size_t>(ST_MAX_CONS, ((size_t)SMEM_OPTIN_MAX - tabb) / per);
-    int NW = 0;
-    double best = 0;
-    for (int w = std::max(1, cap / 2); w <= cap && cap > 0; w++)
-    {
-      const long slots = (long)h->sm_count * w, rounds = (h->S.B + slots - 1) / slots;
-      const double eff = (double)h->S.B / (double)(slots * rounds);
-      if (eff >= best - 1e-12)
-        best = eff, NW = w;
-    }
-    // (a row with fewer chunks than ring stages, i <= 1 or so, is not worth a stream: the register kernel takes it)
-    if (NW >= 1 && NC >= ST_STAGES && (size_t)h->S.ldb * 8 <= ST_STAGE_DBL * sizeof(double) && stream_maps(h, sh.rows_last))
-    {
-      const int ctas = std::min(h->sm_count, (h->S.B + NW - 1) / NW);
-      k_update_row_stream<<<ctas, NW * 32, NW * per + tabb, h->stream>>>(h->S, i, last_j, h->d_ok, h->st_maps);
-      return;
-    }
-  }
-  k_update_row<<<g, t, h->smem_compact, h->stream>>>(h->S, i, last_j, h->d_ok);
+  k_update_row<<<grid_warps(h), WARPS_PER_CTA * 32, h->smem_compact, h->stream>>>(h->S, i, last_j, h->d_ok);
 }
 
 template <class T> static int dev_alloc(b200gso *h, T **p, size_t count)
@@ -577,7 +485,6 @@ int b200gso_create(b200gso_t **out, int batch, int d, int n, int flags, int devi
     return B200GSO_EINVAL;
   }
   const void *fns[] = {(const void *)k_init,         (const void *)k_discover_all, (const void *)k_update_row,
-                       (const void *)k_update_row_stream,
                        (const void *)k_update_gso,   (const void *)k_row_addmul_we, (const void *)k_row_op_end,
                        (const void *)k_row_swap,     (const void *)k_move_row,     (const void *)k_upload_row,
                        (const void *)k_apply_ops,    (const void *)k_upload_row_fp, (const void *)k_init_host_basis};

@@ -6,7 +6,6 @@
 #pragma once
 #include "../../include/b200gso.h"
 #include "gso_lll.cuh"
-#include "gso_stream.cuh"
 #include <cstdio>
 #include <algorithm>
 #include <cstring>
@@ -131,10 +130,7 @@ struct b200gso
   b200gso_op *h_ops;
   size_t h_ops_cap;
   std::vector<void *> allocs;
-  // streaming update kernel (gso_stream.cuh): tensor maps (0 = not built yet, 1 = ready, -1 = unavailable), the row
-  // count the partial-panel maps were encoded for, SMs of the device
-  StreamMaps st_maps;
-  int st_state = 0, st_rows = 0, sm_count = 0;
+  int sm_count = 0;  // SMs of the device: the LLL launcher picks the CTA or the warp kernel by batch size against it
 };
 
 inline int grid_warps(const b200gso *h) { return (h->S.B + WARPS_PER_CTA - 1) / WARPS_PER_CTA; }

@@ -1,8 +1,8 @@
-// tma.cuh — Hopper (sm_90a) bulk-copy and mbarrier primitives for the TMA-fed kernels (k_update_row_stream in
-// gso_stream.cuh, hk_update_R_x32 in hh_api.cu), and the host side that encodes their fp64 tensor maps.
+// tma.cuh — Hopper (sm_90a) tensor-copy and mbarrier primitives for the TMA-fed kernel hk_update_R_x32 (hh_api.cu),
+// and the host side that encodes its fp64 tensor maps.
 //
 // Every barrier here is a CTA-local mbarrier in shared memory (the .shared::cluster destinations of the copies are this
-// CTA's own shared memory: the kernels are launched without clusters).
+// CTA's own shared memory: the kernel is launched without clusters).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -59,25 +59,11 @@ __device__ inline bool tma_mbar_test(unsigned long long *bar, unsigned parity)
 }
 
 // copies global -> shared memory that complete on `bar` (byte count announced with tma_mbar_expect_tx)
-__device__ inline void tma_bulk_1d(void *dst, const void *src, unsigned bytes, unsigned long long *bar)
-{
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                   tma_smem_u32(dst)),
-               "l"(src), "r"(bytes), "r"(tma_smem_u32(bar))
-               : "memory");
-}
 __device__ inline void tma_load_2d(void *dst, const CUtensorMap *map, int c0, int c1, unsigned long long *bar)
 {
   asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::
                    "r"(tma_smem_u32(dst)),
                "l"(map), "r"(c0), "r"(c1), "r"(tma_smem_u32(bar))
-               : "memory");
-}
-__device__ inline void tma_load_3d(void *dst, const CUtensorMap *map, int c0, int c1, int c2, unsigned long long *bar)
-{
-  asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];" ::
-                   "r"(tma_smem_u32(dst)),
-               "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(tma_smem_u32(bar))
                : "memory");
 }
 

@@ -8,7 +8,6 @@ import subprocess
 WANT = ["LDG", "LD", "LDS", "STS", "STG", "DMUL", "DADD", "DFMA", "DMMA", "SHFL", "UTMALDG", "UBLKCP", "UBLKPF", "SYNCS",
         "LDGSTS", "ATOM", "ATOMG", "RED", "REDG", "BAR", "IMAD", "BRA"]
 KERNELS = [("fplll_b200/lib/libb200gso.so", "12k_update_rowE", r"LDG|DMUL|DADD", 8),
-           ("fplll_b200/lib/libb200gso.so", "k_update_row_stream", r"UTMALDG|UBLKCP|SYNCS", 10),
            ("fplll_b200/lib/libb200gso.so", "k_gram_tiles", r"DMMA", 6),
            ("fplll_b200/lib/libb200gso.so", "k_lll_ctaILi8", None, 0),
            ("fplll_b200/lib/libb200hh.so", "hk_update_R_x32", r"UTMALDG|SYNCS", 8),
