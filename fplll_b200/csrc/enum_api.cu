@@ -506,11 +506,15 @@ struct Breadth
 {
   std::vector<std::vector<BNode>> lev;  // lev[t] = accepted nodes of tree level d-1-t; lev[t][0] is the all-zero prefix
   std::vector<uint64_t> nodes;          // d: counted nodes per tree level
+  // level d-1 alone had more candidates than fit: lev[0] holds the first `cap` of them (x = 0 .. cap-1) and the rest,
+  // x = top_rest, top_rest + 1, ..., is left to the device as one task at level d-1 (0: nothing left)
+  int top_rest = 0;
 };
 
-// children of node `pi` of level t-1 at tree level k = d-1-t
+// children of node `pi` of level t-1 at tree level k = d-1-t; stops once `out` holds more than `cap` nodes
 static void expand_children(int d, int k, const double *mut, const double *rdiag, const double *prun, double A, bool dual,
-                            const Breadth &br, int t, int pi, std::vector<BNode> &out, std::vector<double> &chain)
+                            const Breadth &br, int t, int pi, std::vector<BNode> &out, std::vector<double> &chain,
+                            size_t cap)
 {
   // values the chain multiplies with: x_j (primal) or alpha_j (dual) of the ancestors, levels d-1 .. k+1
   int q = pi;
@@ -531,7 +535,7 @@ static void expand_children(int d, int k, const double *mut, const double *rdiag
     BNode z;
     z.pd = 0.0, z.alpha = 0.0, z.parent = pi, z.x = 0;
     out.push_back(z);
-    for (double x = 1.0;; x += 1.0)
+    for (double x = 1.0; out.size() <= cap; x += 1.0)
     {
       const double alphak = x - nc, newdist = pdk + alphak * alphak * rdiag[k];
       if (!(newdist <= prun[k] * A))
@@ -544,7 +548,7 @@ static void expand_children(int d, int k, const double *mut, const double *rdiag
   }
   const double x0 = std::round(nc), s = (nc >= x0) ? 1.0 : -1.0;
   double x = x0;
-  for (int step = 0;; ++step)
+  while (out.size() <= cap)
   {
     const double alphak = x - nc, newdist = pdk + alphak * alphak * rdiag[k];
     if (!(newdist <= prun[k] * A))
@@ -564,6 +568,7 @@ static void breadth_phase(int d, const double *mut, const double *rdiag, const d
 {
   br.lev.clear();
   br.nodes.assign(d, 0);
+  br.top_rest = 0;
   std::vector<double> chain(d + 1, 0.0);
   for (int t = 0; t < d - 1; ++t)
   {
@@ -573,16 +578,21 @@ static void breadth_phase(int d, const double *mut, const double *rdiag, const d
     bool over = false;
     for (size_t pi = 0; pi < np && !over; ++pi)
     {
-      expand_children(d, k, mut, rdiag, prun, A, dual, br, t, (int)pi, cur, chain);
+      expand_children(d, k, mut, rdiag, prun, A, dual, br, t, (int)pi, cur, chain, cap);
       over = cur.size() > cap;
     }
     if (over && t > 0)
       break;  // too many: keep the previous depth
     if (over)
-      cur.resize(cap);  // cannot happen with a sane radius (level d-1 alone has more than `cap` candidates)
+    {
+      // level d-1 alone has more than `cap` candidates (a tiny r(d-1, d-1)): its children of the all-zero root are
+      // x = 0, 1, 2, ... in this order, so the first `cap` become roots and the device walks the rest from one task
+      cur.resize(cap);
+      br.top_rest = cur.back().x + 1;
+    }
     br.nodes[k] = cur.size() - 1;  // the all-zero prefix is not a node
     br.lev.push_back(std::move(cur));
-    if (br.lev.back().size() >= want)
+    if (br.lev.back().size() >= want || br.top_rest)
       break;
   }
 }
@@ -633,8 +643,11 @@ int get_ctx(int device, DevCtx **out)
   CKE(cudaStreamCreateWithFlags(&c.stream, cudaStreamNonBlocking));
   CKE(cudaEventCreate(&c.e0));
   CKE(cudaEventCreate(&c.e1));
-  const size_t cfg_max = ((size_t)B200ENUM_MAX_DIM * B200ENUM_MAX_DIM + 2 * B200ENUM_MAX_DIM) * 8;
-  c.blk_bytes = DevCtx::OFF_STAGE + cfg_max + (size_t)MAX_ROOTS * (sizeof(TaskHdr) + 64 * sizeof(int));
+  // staging: cfg (16-byte aligned), then up to MAX_ROOTS roots plus the task for the rest of a wide level d-1, each
+  // with a prefix row of (d + 3) & ~3 ints — sized for B200ENUM_MAX_DIM (22 MB), so any call's roots fit
+  const size_t cfg_max = (((size_t)B200ENUM_MAX_DIM * B200ENUM_MAX_DIM + 2 * B200ENUM_MAX_DIM) * 8 + 15) & ~(size_t)15;
+  const size_t row_max = (size_t)((B200ENUM_MAX_DIM + 3) & ~3) * sizeof(int);
+  c.blk_bytes = DevCtx::OFF_STAGE + cfg_max + (size_t)(MAX_ROOTS + 1) * (sizeof(TaskHdr) + row_max);
   CKE(cudaMalloc(&c.d_blk, c.blk_bytes));
   CKE(cudaMemset(c.d_blk, 0, DevCtx::OFF_STAGE));
   CKE(cudaMallocHost(&c.h_up, c.blk_bytes));
@@ -839,11 +852,15 @@ int run_impl(int dim, double maxdist, const double *mut_in, const double *rdiag_
   const int T = (int)br.lev.size(), L = d - T;
   const std::vector<BNode> &leaf = br.lev[T - 1];
   const size_t nroots = leaf.size();
-  // roots sorted by partial length (ascending; the all-zero prefix first): most promising subtrees first
-  std::vector<unsigned> order(nroots);
-  for (size_t i = 0; i < nroots; i++)
+  // round-0 tasks: the roots, plus (index nroots) the rest of a level d-1 that had more candidates than MAX_ROOTS
+  const size_t ntask = nroots + (br.top_rest ? 1 : 0);
+  // roots sorted by partial length (ascending; the all-zero prefix first): most promising subtrees first.  The rest of
+  // level d-1 goes last: its nodes are longer than every root's.
+  std::vector<unsigned> order(ntask);
+  for (size_t i = 0; i < ntask; i++)
     order[i] = (unsigned)i;
-  std::stable_sort(order.begin(), order.end(), [&](unsigned a, unsigned b) { return leaf[a].pd < leaf[b].pd; });
+  std::stable_sort(order.begin(), order.begin() + nroots,
+                   [&](unsigned a, unsigned b) { return leaf[a].pd < leaf[b].pd; });
   const auto t_host = std::chrono::steady_clock::now();
 
   // ---- contexts ----
@@ -878,7 +895,7 @@ int run_impl(int dim, double maxdist, const double *mut_in, const double *rdiag_
   // the staged round-0 tasks of this process: its share of the roots
   std::vector<unsigned> mine;
   if (shard_world > 1)
-    for (size_t g = (size_t)shard_rank; g < nroots; g += (size_t)shard_world)
+    for (size_t g = (size_t)shard_rank; g < ntask; g += (size_t)shard_world)
       mine.push_back(order[g]);
   else
     mine = order;
@@ -913,6 +930,15 @@ int run_impl(int dim, double maxdist, const double *mut_in, const double *rdiag_
     std::vector<double> chain(d + 1, 0.0);
     for (size_t g = 0; g < nmine; g++)
     {
+      if (mine[g] == nroots)
+      {
+        // the rest of level d-1: x = top_rest, top_rest + 1, ... under the all-zero prefix (centre 0, and pd = 0 makes
+        // next_sibling step x + 1), each with everything below it
+        TaskHdr h;
+        h.lvl = d - 1, h.pad = 0, h.pd = 0.0, h.cen = 0.0, h.xs = (double)br.top_rest;
+        hdr[g] = h;
+        continue;
+      }
       // the task "level L-1 under this root": prefix x[L..d-1], centre of level L-1 (same chain as the device)
       int q = (int)mine[g];
       int *row = tx + g * (size_t)dstride;
@@ -1219,7 +1245,7 @@ int run_impl(int dim, double maxdist, const double *mut_in, const double *rdiag_
   if (stats)
   {
     stats->host_nodes = host_nodes, stats->device_nodes = dev_nodes, stats->leaves = leaves;
-    stats->top_levels = T, stats->n_roots = (int)nroots, stats->n_solutions = nrep, stats->n_devices = used_dev;
+    stats->top_levels = T, stats->n_roots = (int)ntask, stats->n_solutions = nrep, stats->n_devices = used_dev;
     stats->n_rounds = rounds;
     stats->final_maxdist = cur, stats->device_ms = ms_total;
     stats->host_breadth_us = (float)host_us;

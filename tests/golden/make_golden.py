@@ -409,9 +409,78 @@ def size_class_fixtures():
     np.savez_compressed(os.path.join(HERE, "size_classes_ref.npz"), **pack)
 
 
+def enum_size_inputs():
+    """Bases of enum_size_classes.npz, all from the LLL-reduced r200 basis (r200_lll_update_gso.npz).  An unpruned walk of
+    an 80-row block of it never reaches a leaf in reasonable time, so two 80-row bases get a planted short vector: rows
+    [120, 200) with every row but the first multiplied by 5 (b_0 is the shortest vector, about 8.7e5 nodes away), and the
+    same rows with only the last one multiplied by 5 (the same for the dual, whose first vector is b*_79 / r_79)."""
+    b = np.load(os.path.join(HERE, "r200_lll_update_gso.npz"))["b"]
+    primal, dual = b[120:200].copy(), b[120:200].copy()
+    primal[1:] *= 5
+    dual[-1] *= 5
+    return dict(r200=b, plant_primal=primal, plant_dual=dual)
+
+
+# (name, basis, FIRST, LAST, FACTOR, pruning, ref_probe mode).  The radius is FACTOR * r(FIRST, FIRST), or FACTOR /
+# r(LAST-1, LAST-1) for the dual; with these factors each of the reference's walks visits 2e5-1.5e6 nodes, well under
+# a second.
+ENUM_SIZE_CASES = [
+    ("p80", "plant_primal", 0, 80, 1.01, None, "capture"),
+    ("dual80", "plant_dual", 0, 80, 1.01, None, "capture_dual"),
+    ("subsols80", "plant_primal", 0, 80, 1.01, None, "capture_subsols"),
+    ("p100", "r200", 100, 200, 0.01, "strategy100", "capture"),
+    ("p160", "r200", 40, 200, 1e-4, "linear", "capture"),
+]
+
+
+def enum_size_pruning(kind, d):
+    """strategy100: the beta = 100 coefficients of strategies/default.json for the GH factor 1.0; linear: (d - i) / d."""
+    if kind == "strategy100":
+        z = np.load(os.path.join(os.path.dirname(os.path.dirname(HERE)), "fplll_b200", "data", "strategies_default.npz"))
+        ghf = z["ghf_100"]
+        return np.ascontiguousarray(z["coef_100"][int(np.argmin(np.abs(ghf - 1.0)))], np.float64)
+    return (d - np.arange(d)) / float(d)
+
+
+def enum_size_fixtures():
+    """tests/golden/enum_size_classes.npz (python tests/golden/make_golden.py --enum-sizes, about a second): the reference's
+    own enumerator above 64 dimensions through the capture hook (what the plugin API hands an external enumerator, then
+    the internal enumerator runs) on ENUM_SIZE_CASES: the hook's mut / rdiag / pruning / radius, and the reference's
+    per-level nodes, best vector and, for sub-solutions, the per-level best partial vectors."""
+    bases = enum_size_inputs()
+    out = os.path.join(TMP, "enum_size_fixture.bin")
+    if os.path.exists(out):
+        os.remove(out)
+    script = []
+    for name, base, first, last, factor, prune, mode in ENUM_SIZE_CASES:
+        mat = os.path.join(TMP, "enum_size_%s.txt" % base)
+        O.write_matrix(mat, bases[base])
+        pf = "-"
+        if prune:
+            pf = os.path.join(TMP, "enum_size_%s.prune" % name)
+            open(pf, "w").write(" ".join(repr(float(c)) for c in enum_size_pruning(prune, last - first)))
+        script.append("load %s\ntolong\ngso l 2\nupdate_gso\nenum %d %d %r %s %s %s\n" % (mat, first, last, factor, pf,
+                                                                                         out, mode))
+    print(O.run_ref("".join(script), timeout=600))
+    recs = O.read_enum_records(out)
+    arrs = {}
+    for (name, *_), r in zip(ENUM_SIZE_CASES, recs):
+        arrs.update({name + "_mut": r["mut"], name + "_rdiag": r["rdiag"], name + "_pruning": r["pruning"],
+                     name + "_maxdist": np.float64(r["maxdist"]), name + "_normexp": np.int64(r["normexp"]),
+                     name + "_found": np.int32(r["found"]), name + "_best": np.float64(r["best"]),
+                     name + "_sol": r["sol"], name + "_nodes": r["nodes"]})
+        if r["subsols"]:
+            arrs[name + "_subdist"] = r["subdist"]
+            arrs[name + "_subsol"] = r["subsol"]
+        print(name, "d", len(r["rdiag"]), "found", r["found"], "nodes", int(r["nodes"].sum()), flush=True)
+    np.savez_compressed(os.path.join(HERE, "enum_size_classes.npz"), **arrs)
+
+
 if __name__ == "__main__":
     if "--sizes" in sys.argv:
         size_class_fixtures()
+    elif "--enum-sizes" in sys.argv:
+        enum_size_fixtures()
     elif "--live" in sys.argv:
         live_fixtures()
     elif "--config2" in sys.argv:

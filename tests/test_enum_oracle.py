@@ -70,3 +70,28 @@ def test_oracle_dual_and_subsolutions_match_reference():
         if subs:
             assert np.array_equal(np.where(res["subdist"] > 0, res["subdist"] * 2.0 ** ne, -1.0), z[name + "_subdist"])
             assert np.array_equal(res["subsol"], z[name + "_subsol"])
+
+
+ENUM_SIZE_CASES = (("p80", False, False), ("dual80", True, False), ("subsols80", False, True), ("p100", False, False),
+                   ("p160", False, False))
+
+
+def test_oracle_matches_reference_above_64_dimensions():
+    """The reference's own enumerator on blocks of 80, 100 and 160 dimensions (tests/golden/enum_size_classes.npz, made
+    by make_golden.py --enum-sizes): unpruned primal, dual and sub-solution walks that find a planted shortest vector at
+    d = 80, and pruned walks at d = 100 (beta = 100 strategy coefficients) and d = 160 (linear profile)."""
+    z = H.gold("enum_size_classes.npz")
+    for name, dual, subs in ENUM_SIZE_CASES:
+        res = O.enum_svp_ex(z[name + "_mut"], z[name + "_rdiag"], z[name + "_pruning"], float(z[name + "_maxdist"]),
+                            dual=dual, findsubsols=subs)
+        ne = int(z[name + "_normexp"])
+        assert len(res["nodes"]) == len(z[name + "_rdiag"]) > 64, name
+        assert np.array_equal(res["nodes"], z[name + "_nodes"]), name
+        assert (res["nsols"] > 0) == bool(z[name + "_found"]), name
+        if res["nsols"]:
+            assert res["best"] * 2.0 ** ne == float(z[name + "_best"]), name
+            assert np.array_equal(res["sol"], z[name + "_sol"]), name
+        if subs:
+            assert np.array_equal(np.where(res["subdist"] > 0, res["subdist"] * 2.0 ** ne, -1.0), z[name + "_subdist"])
+            assert np.array_equal(res["subsol"], z[name + "_subsol"])
+            assert (z[name + "_subdist"] > 0).sum() > 10
