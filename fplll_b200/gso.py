@@ -9,6 +9,9 @@ from ._lib import B200Error, load
 
 GSO_DEFAULT, GSO_INT_GRAM, GSO_ROW_EXPO, GSO_OP_FORCE_LONG = 0, 1, 2, 4  # gso_interface.h:26-32
 RED_SUCCESS, RED_GSO_FAILURE, RED_BABAI_FAILURE, RED_LLL_FAILURE = 0, 2, 3, 4  # defs.h:153-169
+# b200gso_op types (include/b200gso.h)
+OP_ROW_ADDMUL, OP_MOVE_ROW, OP_ROW_SWAP, OP_ROW_OP_END, OP_NEGATE = 1, 2, 3, 4, 5
+_OP_DTYPE = np.dtype([("type", np.int32), ("a", np.int32), ("b", np.int32), ("pad", np.int32), ("x", np.float64)])
 
 _P = C.POINTER
 _sig_done = False
@@ -201,12 +204,34 @@ class MatGSO:
         return self.state()["r"]
 
     # ---- device LLL ----------------------------------------------------------------------------------
-    def lll(self, delta=0.99, eta=0.51):
-        """LLLReduction(m, delta, eta, LLL_DEFAULT).lll() on every lattice; returns (status[batch], stats)."""
+    def lll(self, delta=0.99, eta=0.51, kappa_min=0, kappa_start=0, kappa_end=-1, size_reduction_start=0):
+        """LLLReduction(m, delta, eta, LLL_DEFAULT).lll(kappa_min, kappa_start, kappa_end, size_reduction_start) on every
+        lattice; returns (status[batch], stats)."""
         st = np.zeros(self.batch, np.int32)
         stats = np.zeros((self.batch, 4), np.int64)
-        _ck(_lib().b200gso_lll(self._h, delta, eta, _ptr(st, C.c_int), _ptr(stats, C.c_long)), "lll")
+        if (kappa_min, kappa_start, kappa_end, size_reduction_start) == (0, 0, -1, 0):
+            _ck(_lib().b200gso_lll(self._h, delta, eta, _ptr(st, C.c_int), _ptr(stats, C.c_long)), "lll")
+        else:
+            _ck(_lib().b200gso_lll_range(self._h, delta, eta, kappa_min, kappa_start, kappa_end, size_reduction_start,
+                                         _ptr(st, C.c_int), _ptr(stats, C.c_long)), "lll")
         return st, dict(n_swaps=stats[:, 0], final_kappa=stats[:, 1], zeros=stats[:, 2], babai_iters=stats[:, 3])
+
+    def size_reduction(self, eta=0.51, kappa_min=0, kappa_end=-1, size_reduction_start=0):
+        """LLLReduction(m, 0.99, eta, LLL_DEFAULT).size_reduction(kappa_min, kappa_end, size_reduction_start) on every
+        lattice; returns status[batch] (RED_GSO_FAILURE where the reference returns false without a status)."""
+        st = np.zeros(self.batch, np.int32)
+        _ck(_lib().b200gso_size_reduction(self._h, eta, kappa_min, kappa_end, size_reduction_start, _ptr(st, C.c_int)),
+            "size_reduction")
+        return st
+
+    def apply_ops(self, ops):
+        """Runs a list of (type, a, b, x) in one launch on every lattice (b200gso_apply_ops): OP_ROW_ADDMUL
+        row_addmul(a, b, x), OP_MOVE_ROW move_row(a, b), OP_ROW_SWAP row_swap(a, b), OP_ROW_OP_END row_op_end(a, b),
+        OP_NEGATE negate_row_of_b(a)."""
+        arr = np.zeros(len(ops), _OP_DTYPE)
+        for k, (t, a, b, x) in enumerate(ops):
+            arr[k] = (t, a, b, 0, x)
+        _ck(_lib().b200gso_apply_ops(self._h, arr.ctypes.data_as(C.c_void_p), len(ops)), "apply_ops")
 
     def time_update_row(self, i, reps, invalidate=True):
         """returns (mean ms of one update_gso_row launch, total ms of the `reps` steps), CUDA events on the handle's stream"""

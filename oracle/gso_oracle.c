@@ -510,22 +510,30 @@ static long get_max_exp_of_b(ogso_t *m) /* Matrix::get_max_exp, Z_NR<long>::expo
   return mx;
 }
 
-/* LLLReduction::lll, lll.cpp:44-164 (no early reduction, no siegel, kappa_min=kappa_start=0, full range) */
-int ogso_lll(ogso_t *m, olll_t *L)
+/* LLLReduction::lll(kappa_min, kappa_start, kappa_end, size_reduction_start), lll.cpp:44-164, with LLL_DEFAULT flags
+ * (no early reduction, no siegel).  kappa_end = -1 stands for d (lll.cpp:48-49).  Returns the reference's bool; L->status
+ * is only written where the reference calls set_status, so a caller starts it at ORED_SUCCESS like the constructor
+ * (lll.cpp:28-29) and the one early `return false` that sets no status (update_gso_row failing at kappa_start,
+ * lll.cpp:71-76) leaves it there. */
+int ogso_lll_range(ogso_t *m, olll_t *L, int kappa_min, int kappa_start, int kappa_end, int sr_start)
 {
-  int d = m->d, kappa_end = d, kappa = 1;
-  double *lov = (double *)calloc(d + 1, sizeof(double)), *bmu = (double *)calloc(d, sizeof(double));
-  long *bex   = (long *)calloc(d, sizeof(long));
+  if (kappa_end == -1)
+    kappa_end = m->d;
+  int d = kappa_end - kappa_min, kappa = kappa_start + 1, ok = 0;
+  double *lov = (double *)calloc(kappa_end + 1, sizeof(double));
+  double *bmu = (double *)calloc(kappa_end + 1, sizeof(double));
+  long *bex   = (long *)calloc(kappa_end + 1, sizeof(long));
   L->swap_threshold = L->delta;
   L->zeros = L->n_swaps = L->final_kappa = 0;
   L->n_babai_iters = L->n_row_ops = 0;
-  L->status                       = -1;
+  /* row 0 is tested, row kappa_min is moved: the reference's own loop (lll.cpp:66-69) */
   for (; L->zeros < d && b_row_is_zero(m, 0); L->zeros++)
-    ogso_move_row(m, 0, kappa_end - 1 - L->zeros);
-  if (L->zeros < d && !ogso_update_gso_row(m, 0, 0))
+    ogso_move_row(m, kappa_min, kappa_end - 1 - L->zeros);
+  if (L->zeros < d && ((kappa_start > 0 && !ogso_babai(m, L, kappa_start, kappa_start, sr_start, bmu, bex)) ||
+                       !ogso_update_gso_row(m, kappa_start, kappa_start)))
   {
-    L->final_kappa = 0;
-    goto out; /* status stays as set by caller convention: GSO failure path returns false without status */
+    L->final_kappa = kappa_start;
+    goto out;
   }
   {
     long long max_iter =
@@ -533,7 +541,7 @@ int ogso_lll(ogso_t *m, olll_t *L)
     long long iter;
     for (iter = 0; iter < max_iter && kappa < kappa_end - L->zeros; iter++)
     {
-      if (!ogso_babai(m, L, kappa, kappa, 0, bmu, bex))
+      if (!ogso_babai(m, L, kappa, kappa, sr_start, bmu, bex))
       {
         L->final_kappa = kappa;
         goto out;
@@ -551,7 +559,7 @@ int ogso_lll(ogso_t *m, olll_t *L)
       {
         L->n_swaps++;
         int old_k = kappa;
-        for (kappa--; kappa > 0; kappa--)
+        for (kappa--; kappa > kappa_min; kappa--)
         {
           double t2 = R(kappa - 1, kappa - 1) * L->swap_threshold;
           if (m->enable_row_expo)
@@ -573,8 +581,34 @@ int ogso_lll(ogso_t *m, olll_t *L)
       kappa++;
     }
     L->status = (kappa < kappa_end - L->zeros) ? ORED_LLL_FAILURE : ORED_SUCCESS;
+    ok        = L->status == ORED_SUCCESS;
   }
 out:
   free(lov), free(bmu), free(bex);
-  return L->status == ORED_SUCCESS;
+  return ok;
+}
+
+/* LLLReduction::size_reduction(kappa_min, kappa_end, size_reduction_start), lll.h:106-122.  Returns the reference's
+ * bool; L->status as in ogso_lll_range (a failing update_gso_row returns false without a status, lll.h:118-119). */
+int ogso_size_reduction(ogso_t *m, olll_t *L, int kappa_min, int kappa_end, int sr_start)
+{
+  if (kappa_end == -1)
+    kappa_end = m->d;
+  double *bmu = (double *)calloc(kappa_end + 1, sizeof(double));
+  long *bex   = (long *)calloc(kappa_end + 1, sizeof(long));
+  int ok      = 1;
+  for (int k = kappa_min; k < kappa_end && ok; k++)
+    if ((k > 0 && !ogso_babai(m, L, k, k, sr_start, bmu, bex)) || !ogso_update_gso_row(m, k, k))
+      ok = 0;
+  if (ok)
+    L->status = ORED_SUCCESS;
+  free(bmu), free(bex);
+  return ok;
+}
+
+/* MatGSO::negate_row_of_b, gso.h:291-297 (no integer Gram matrix: the integer row only) */
+void ogso_negate_row_of_b(ogso_t *m, int i)
+{
+  for (int c = 0; c < m->n; c++)
+    B(i, c) = (int64_t)(0 - (uint64_t)B(i, c));
 }

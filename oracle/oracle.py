@@ -70,7 +70,9 @@ def lib():
         L.ogso_get_gram.restype = C.c_double
         L.ogso_rnd_we.argtypes = [C.c_double, C.c_long]
         L.ogso_rnd_we.restype = C.c_double
-        L.ogso_lll.argtypes = [C.POINTER(_OGSO), C.POINTER(_OLLL)]
+        L.ogso_lll_range.argtypes = [C.POINTER(_OGSO), C.POINTER(_OLLL), C.c_int, C.c_int, C.c_int, C.c_int]
+        L.ogso_size_reduction.argtypes = [C.POINTER(_OGSO), C.POINTER(_OLLL), C.c_int, C.c_int, C.c_int]
+        L.ogso_negate_row_of_b.argtypes = [C.POINTER(_OGSO), C.c_int]
         L.ogso_babai.argtypes = [C.POINTER(_OGSO), C.POINTER(_OLLL), C.c_int, C.c_int, C.c_int,
                                  C.POINTER(C.c_double), C.POINTER(C.c_long)]
         _lib = L
@@ -116,14 +118,34 @@ class OracleGSO:
     def set_r(self, i, j, f):
         lib().ogso_set_r(self._p, i, j, float(f))
 
+    def negate_row_of_b(self, i):
+        lib().ogso_negate_row_of_b(self._p, i)
+
+    def upload_row(self, i, row):
+        """What b200gso_upload_row does to one lattice: b[i] = row, then row_op_end(i, i+1)."""
+        row = np.ascontiguousarray(row, dtype=np.int64)
+        assert row.shape == (self.n,)
+        C.memmove(C.addressof(self._p.contents.b.contents) + 8 * i * self.n, row.ctypes.data, 8 * self.n)
+        self.row_op_end(i, i + 1)
+
     def get_gram(self, i, j):
         return lib().ogso_get_gram(self._p, i, j)
 
-    def lll(self, delta=0.99, eta=0.51):
+    def lll(self, delta=0.99, eta=0.51, kappa_min=0, kappa_start=0, kappa_end=-1, size_reduction_start=0):
+        """LLLReduction(m, delta, eta, LLL_DEFAULT).lll(kappa_min, kappa_start, kappa_end, size_reduction_start) on a
+        fresh LLLReduction object: `ok` is the reference's return value, `status` its status member, which starts at
+        RED_SUCCESS (lll.cpp:28-29) and stays there when update_gso_row fails at kappa_start (lll.cpp:71-76)."""
         L = _OLLL(delta=delta, eta=eta)
-        lib().ogso_lll(self._p, C.byref(L))
-        return dict(status=L.status, n_swaps=L.n_swaps, final_kappa=L.final_kappa, zeros=L.zeros,
+        ok = lib().ogso_lll_range(self._p, C.byref(L), kappa_min, kappa_start, kappa_end, size_reduction_start)
+        return dict(ok=bool(ok), status=L.status, n_swaps=L.n_swaps, final_kappa=L.final_kappa, zeros=L.zeros,
                     n_babai_iters=L.n_babai_iters, n_row_ops=L.n_row_ops)
+
+    def size_reduction(self, eta=0.51, kappa_min=0, kappa_end=-1, size_reduction_start=0):
+        """LLLReduction(m, 0.99, eta, LLL_DEFAULT).size_reduction(kappa_min, kappa_end, size_reduction_start) on a fresh
+        LLLReduction object (lll.h:106-122): `ok` and `status` as in lll()."""
+        L = _OLLL(delta=0.99, eta=eta)
+        ok = lib().ogso_size_reduction(self._p, C.byref(L), kappa_min, kappa_end, size_reduction_start)
+        return dict(ok=bool(ok), status=L.status)
 
     # -- state views (copies) -----------------------------------------------------------------------------
     def _arr(self, ptr, shape, dt):

@@ -407,7 +407,8 @@ int main(int argc, char **argv)
     {
       puts("load P | save P | tolong | gso l|m FLAGS | update_gso | update_row I J | discover_all | "
            "row_addmul_we I J X E | row_op_begin F L | row_op_end F L | move_row O N | row_swap I J | "
-           "set_r I J V | dump P | dumpb P | lll DELTA ETA METHOD FLOAT FLAGS | islll DELTA ETA | "
+           "set_r I J V | dump P | dumpb P | lll DELTA ETA METHOD FLOAT FLAGS | lll_range DELTA ETA KMIN KSTART KEND SRSTART | "
+           "size_reduction ETA KMIN KEND SRSTART | islll DELTA ETA | "
            "bkz BLOCK FLAGS MAXLOOPS default|none internal|enumlib THREADS | enum FIRST LAST FACTOR PRUNEFILE OUT internal|enumlib|capture | set_threads T | time_update_row I REPS INV | time_update_row_mt I REPS T PER | time_update_gso_mt REPS T PER");
     }
     else if (c == "load")
@@ -580,6 +581,27 @@ int main(int argc, char **argv)
       double t0 = now();
       lll.lll();
       printf("lll_long status=%d sec=%.6f swaps=%d\n", lll.status, now() - t0, lll.n_swaps);
+    }
+    else if (c == "lll_range" || c == "size_reduction")
+    {
+      /* lll_range DELTA ETA KMIN KSTART KEND SRSTART | size_reduction ETA KMIN KEND SRSTART : a fresh
+         LLLReduction<Z_NR<long>, FP_NR<double>> (LLL_DEFAULT) on the current long GSO object, so that its status starts
+         at RED_SUCCESS (lll.cpp:28-29); prints the return value, status, swaps, final_kappa and zeros */
+      double delta = 0.99, eta;
+      int kmin, kstart = 0, kend, srs;
+      if (c == "lll_range")
+        is >> delta >> eta >> kmin >> kstart >> kend >> srs;
+      else
+        is >> eta >> kmin >> kend >> srs;
+      if (!gl)
+      {
+        fprintf(stderr, "%s needs a long GSO\n", c.c_str());
+        return 2;
+      }
+      LLLReduction<Z_NR<long>, FP_NR<double>> red(*gl, delta, eta, LLL_DEFAULT);
+      bool ok = c == "lll_range" ? red.lll(kmin, kstart, kend, srs) : red.size_reduction(kmin, kend, srs);
+      printf("%s ok=%d status=%d swaps=%d final_kappa=%d zeros=%d\n", c.c_str(), (int)ok, red.status, red.n_swaps,
+             red.final_kappa, red.zeros);
     }
     else if (c == "islll")
     {

@@ -476,9 +476,62 @@ def enum_size_fixtures():
     np.savez_compressed(os.path.join(HERE, "enum_size_classes.npz"), **arrs)
 
 
+# (seed, d, bits, calls) of lll_ranged_ref.npz: full state dumps after every call at d <= 64, digests at d = 300
+RANGED_CASES = [(11, 20, 10, 14), (12, 40, 12, 12), (13, 300, 12, 8)]
+
+
+def ranged_fixtures():
+    """tests/golden/lll_ranged_ref.npz (python tests/golden/make_golden.py --ranged): the reference's
+    LLLReduction<Z_NR<long>, FP_NR<double>>::lll(kappa_min, kappa_start, kappa_end, size_reduction_start) and
+    size_reduction on one MatGSO<long, double> object (GSO_ROW_EXPO) driven through helpers.ranged_call_script.  Per case:
+    the input, the script, per call (ok, status, swaps, final_kappa, zeros) and a digest of the state (helpers.gso_digest);
+    at d <= 64 also the state after every call (entries the reference leaves undefined are zeroed), at d = 300 the final
+    basis."""
+    import json
+    pack = {}
+    for case, (seed, d, bits, calls) in enumerate(RANGED_CASES):
+        b = H.ranged_inputs(seed, d, bits)
+        ops = H.ranged_call_script(np.random.default_rng(seed), d, calls)
+        s = O.RefSession(b)
+        for op in ops:
+            s.lines += H.ranged_ref_lines(op)
+            if op[0] in ("lll", "sr"):
+                s.dump_state()
+        out, recs = s.run()
+        res = [[int(t.split("=")[1]) for t in line.split()[1:]] for line in out.splitlines()
+               if line.startswith(("lll_range ", "size_reduction "))]
+        assert len(res) == len(recs) == sum(op[0] in ("lll", "sr") for op in ops)
+        p = "c%d_" % case
+        pack[p + "b"] = _narrow(b)
+        pack[p + "ops_json"] = np.frombuffer(json.dumps(ops).encode(), dtype=np.uint8)
+        pack[p + "res"] = np.array(res, np.int32)
+        pack[p + "digest"] = np.array([H.gso_digest(r) for r in recs])
+        if d <= 64:
+            for key in ["n_known_rows", "n_known_cols", "n_source_rows"]:
+                pack[p + "s_" + key] = np.array([r[key] for r in recs], np.int32)
+            for key in ["row_expo", "gso_valid_cols", "init_row_size", "b", "bf", "gf", "mu", "r"]:
+                arrs = []
+                for r in recs:
+                    a = r[key].copy()
+                    if key in ("mu", "r", "gf"):
+                        keep = np.zeros(a.shape, bool)
+                        for i in range(r["n_known_rows"]):
+                            v = int(r["gso_valid_cols"][i])
+                            keep[i, : {"mu": min(v, i), "r": v, "gf": i + 1}[key]] = True
+                        a[~keep] = 0.0
+                    arrs.append(a)
+                pack[p + "s_" + key] = _narrow(np.array(arrs)) if key == "b" else np.array(arrs)
+        else:
+            pack[p + "b_out"] = _narrow(recs[-1]["b"])
+        print("case", case, "d", d, "calls", len(res), "results", res, flush=True)
+    np.savez_compressed(os.path.join(HERE, "lll_ranged_ref.npz"), **pack)
+
+
 if __name__ == "__main__":
     if "--sizes" in sys.argv:
         size_class_fixtures()
+    elif "--ranged" in sys.argv:
+        ranged_fixtures()
     elif "--enum-sizes" in sys.argv:
         enum_size_fixtures()
     elif "--live" in sys.argv:

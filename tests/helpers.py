@@ -185,3 +185,139 @@ def ops_to_ref_script(ops):
         else:
             lines.append(" ".join(str(x) for x in op))
     return lines
+
+
+def gso_digest(s):
+    """sha256 over the MatGSO state entries assert_state_equal compares (NaN canonical)."""
+    import hashlib
+    h = hashlib.sha256()
+    nkr = int(s["n_known_rows"])
+    h.update(np.array([nkr, int(s["n_known_cols"]), int(s["n_source_rows"])], np.int64).tobytes())
+    h.update(np.ascontiguousarray(s["gso_valid_cols"][:nkr], np.int64).tobytes())
+    for k in ["init_row_size", "row_expo", "b"]:
+        h.update(np.ascontiguousarray(s[k], np.int64).tobytes())
+    h.update(_f64_bytes(s["bf"]))
+    for i in range(nkr):
+        v = int(s["gso_valid_cols"][i])
+        h.update(_f64_bytes(s["gf"][i, : i + 1]) + _f64_bytes(s["mu"][i, : min(v, i)]) + _f64_bytes(s["r"][i, :v]))
+    return h.hexdigest()
+
+
+def ranged_inputs(seed, d, bits):
+    """A (d, d + 1) basis for ranged_call_script: uniform `bits`-bit rows, the last three of them very short (entries in
+    [-2, 2]): the rows that the script's insertions move into the reduced part one after the other."""
+    rng = np.random.default_rng(seed)
+    b = rng.integers(-(1 << bits), 1 << bits, size=(d, d + 1), dtype=np.int64)
+    b[d - 3:] = rng.integers(-2, 3, size=(3, d + 1))
+    return b
+
+
+def _range_edges(d):
+    return [e for e in (2, 3, 31, 32, 33, 63, 64, 65, 255, 256, 257) if e < d] + [d]
+
+
+def ranged_call_script(rng, d, n_calls):
+    """A seeded script of LLLReduction calls and row mutations in the style of the BKZ driver (bkz.cpp): ranged
+    lll(kappa_min, kappa_start, kappa_end, size_reduction_start) and size_reduction calls with range ends on the
+    32-row panel edges, delta / eta changes, and row_addmul, row_swap and move_row insertions of the short rows that
+    ranged_inputs plants at the end (while no call has reached them).  The script keeps to what the reference asks of
+    its callers: before a call that starts above row 0 the rows below its start get a valid GSO (update_gso_row), and
+    a row is discovered before move_row moves it down.  Entries are JSON-friendly lists:
+      ["lll", delta, eta, kmin, kstart, kend, srs], ["sr", eta, kmin, kend, srs], ["addmul", i, j, x],
+      ["swap", i, j], ["move", old, new], ["discover_all"], ["update_rows", k] (update_gso_row(t, t) for t < k)."""
+    edges = _range_edges(d)
+    first = [e for e in edges if e < d - 3]  # the planted rows stay out of the first reduction
+    ops = [["lll", 0.99, 0.51, 0, 0, int(rng.choice(first[len(first) // 2:])), 0]]
+    delta, eta, inserted, reached = 0.99, 0.51, 0, ops[0][5]
+    for _ in range(n_calls):
+        u = rng.random()
+        if u < 0.1:
+            delta, eta = [(0.99, 0.51), (0.75, 0.51), (0.99, 0.6), (0.999, 0.501)][int(rng.integers(0, 4))]
+        kend = int(rng.choice(edges)) if rng.random() < 0.7 else int(rng.integers(2, d + 1))
+        if u < 0.5:
+            shape = int(rng.integers(0, 4))
+            if shape == 0:  # lll(0, 0, kend): the resuming prefix call of svp_preprocessing
+                kmin = kstart = 0
+            elif shape == 1:  # lll(k, k, kend): BKZ_BOUNDED_LLL and slide reduction
+                kmin = kstart = int(rng.integers(0, kend - 1))
+            else:  # kappa_start > kappa_min
+                kmin = int(rng.integers(0, kend - 1))
+                kstart = int(rng.integers(kmin, kend))
+            srs = [0, 0, int(rng.integers(0, kmin + 1)), int(rng.integers(kmin, kend)), kstart][int(rng.integers(0, 5))]
+            if kstart:
+                ops.append(["update_rows", kstart])
+            ops.append(["lll", delta, eta, kmin, kstart, -1 if kend == d and rng.random() < 0.5 else kend, srs])
+            reached = max(reached, kend)
+        elif u < 0.65:
+            kmin = int(rng.integers(0, kend + 1))
+            srs = [0, 0, int(rng.integers(0, kmin + 1)), max(0, kmin - 2)][int(rng.integers(0, 4))]
+            if kmin:
+                ops.append(["update_rows", kmin])
+            ops.append(["sr", eta, kmin, kend, srs])
+            reached = max(reached, kend)
+        elif u < 0.8:
+            i = int(rng.integers(1, d - 3))
+            ops.append(["addmul", i, int(rng.integers(0, i)), float(rng.choice([-2, -1, 1, 3]))])
+        elif u < 0.9 and reached <= d - 3 + inserted:
+            # BKZ's insertion (bkz.cpp svp_postprocessing): a new row moved to kappa, then lll(kappa, kappa, kappa + beta)
+            k = int(rng.integers(0, reached))
+            ops += [["discover_all"], ["move", d - 1, k]]
+            inserted += 1
+            kend = int(min(d - 3 + inserted, k + rng.integers(2, 40)))
+            reached = max(reached, kend)
+            if k:
+                ops.append(["update_rows", k])
+            ops.append(["lll", delta, eta, k, k, kend, 0])
+        else:
+            i, j = (int(x) for x in rng.choice(d - 3, 2, replace=False))
+            ops.append(["swap", i, j])
+    ops.append(["lll", 0.99, 0.51, 0, 0, d, 0])
+    return ops
+
+
+def ranged_apply(m, op):
+    """Runs one entry of ranged_call_script on an OracleGSO or a fplll_b200.MatGSO; returns what lll / size_reduction
+    return, None for the mutations."""
+    k, a = op[0], op[1:]
+    if k == "lll":
+        return m.lll(*a)
+    if k == "sr":
+        return m.size_reduction(*a)
+    if k == "addmul":
+        m.row_addmul_we(a[0], a[1], a[2], 0)
+        m.row_op_end(a[0], a[0] + 1)
+    elif k == "swap":
+        m.row_swap(a[0], a[1])
+        m.row_op_end(min(a), max(a) + 1)
+    elif k == "move":
+        m.move_row(a[0], a[1])
+    elif k == "discover_all":
+        m.discover_all_rows()
+    elif k == "update_rows":
+        for t in range(a[0]):
+            m.update_gso_row(t, t)
+    else:
+        raise ValueError(k)
+    return None
+
+
+def ranged_ref_lines(op):
+    """The ref_probe commands of one ranged_call_script entry (oracle/ref_probe.cpp)."""
+    k, a = op[0], op[1:]
+    if k == "lll":
+        return ["lll_range %r %r %d %d %d %d" % tuple(a)]
+    if k == "sr":
+        return ["size_reduction %r %d %d %d" % tuple(a)]
+    if k == "addmul":
+        return ["row_op_begin %d %d" % (a[0], a[0] + 1), "row_addmul_we %d %d %r 0" % tuple(a),
+                "row_op_end %d %d" % (a[0], a[0] + 1)]
+    if k == "swap":
+        lo, hi = min(a), max(a) + 1
+        return ["row_op_begin %d %d" % (lo, hi), "row_swap %d %d" % tuple(a), "row_op_end %d %d" % (lo, hi)]
+    if k == "move":
+        return ["move_row %d %d" % tuple(a)]
+    if k == "discover_all":
+        return ["discover_all"]
+    if k == "update_rows":
+        return ["update_row %d %d" % (t, t) for t in range(a[0])]
+    raise ValueError(k)

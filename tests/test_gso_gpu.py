@@ -190,53 +190,18 @@ def test_device_lll_wide_vs_oracle(fb, lll_mode, seed, d, bits):
 
 
 def test_ranged_lll_and_size_reduction_resume_are_exact(fb, lll_mode):
-    """lll(0,0,k) / size_reduction(0,k) resume after the clean prefix; the result must equal a from-scratch oracle run
-    of the same call sequence (BKZ's pattern: reduce a prefix, touch a row, reduce a longer prefix)."""
-    import ctypes as C
-    from fplll_b200.gso import _lib, _ck, _ptr
+    """lll(0,0,k) / size_reduction(0,k) resume after the clean prefix (BKZ's pattern: reduce a prefix, touch a row,
+    reduce a longer prefix).  Status, n_swaps, zeros, final_kappa and the whole state after every call must equal the
+    ranged oracle's on the same continuing object."""
+    from test_lll_ranged_gpu import Pair
     rng = np.random.default_rng(41)
     d = 60
-    b = rng.integers(-(1 << 12), 1 << 12, size=(d, d), dtype=np.int64)
-    md, mo = fb.MatGSO(b), O.OracleGSO(b)
-    st = np.zeros(1, np.int32)
-
-    def dev_lll(kend):
-        _ck(_lib().b200gso_lll_range(md._h, 0.99, 0.51, 0, 0, kend, 0, _ptr(st, C.c_int), None), "lll_range")
-        return int(st[0])
-
-    def dev_sr(kend):
-        _ck(_lib().b200gso_size_reduction(md._h, 0.51, 0, kend, 0, _ptr(st, C.c_int)), "size_reduction")
-        return int(st[0])
-    L = O.lib()
-    olll = O._OLLL(delta=0.99, eta=0.51)
-
-    def ora_lll(kend):
-        # oracle: full-range restatement only covers (0,0,d); emulate lll(0,0,kend) on a truncated view by running the
-        # reference semantics through babai + Lovasz on rows < kend: use a fresh oracle on the first kend rows
-        sub = O.OracleGSO(mo.state()["b"][:kend])
-        r = sub.lll(0.99, 0.51)
-        bb = mo.state()["b"].copy()
-        bb[:kend] = sub.state()["b"]
-        return r["status"], bb
-    # sequence: lll(30) ; lll(45) ; modify row 20 ; lll(60)
-    assert dev_lll(30) == 0
-    s1, bb = ora_lll(30)
-    mo = O.OracleGSO(bb)
-    assert np.array_equal(md.b[0], bb)
-    assert dev_lll(45) == 0
-    s2, bb = ora_lll(45)
-    mo = O.OracleGSO(bb)
-    assert np.array_equal(md.b[0], bb)
-    md.row_addmul_we(20, 3, 7.0, 0)
-    md.row_op_end(20, 21)
-    mo.row_addmul_we(20, 3, 7.0, 0)
-    mo.row_op_end(20, 21)
-    assert dev_sr(40) == 0
-    assert dev_lll(60) == 0
-    s3, bb = ora_lll(60)
-    assert np.array_equal(md.b[0], bb)
-
-
+    p = Pair(fb, rng.integers(-(1 << 12), 1 << 12, size=(1, d, d), dtype=np.int64))
+    p.lll(kend=30)
+    p.lll(kend=45)
+    p.run([["addmul", 20, 3, 7.0]])
+    p.sr(kend=40)
+    p.lll(kend=60)
 
 
 @pytest.mark.parametrize("mode", [0, 1])

@@ -100,3 +100,32 @@ def test_ragged_and_zero_rows_live():
     H.assert_state_equal(m.state(), _state_from_npz(z, "ragged0_"), "partial")
     m.move_row(1, 9)
     H.assert_state_equal(m.state(), _state_from_npz(z, "ragged1_"), "after move_row beyond known rows")
+
+
+@pytest.mark.parametrize("case", [0, 1, 2])
+def test_ranged_lll_scripts_match_reference(case):
+    """LLLReduction::lll(kappa_min, kappa_start, kappa_end, size_reduction_start) and size_reduction on one continuing
+    object: every call of the seeded scripts of tests/golden/lll_ranged_ref.npz (make_golden.py --ranged) must return
+    the reference's ok, status, swaps, final_kappa and zeros and leave its state (full dumps at d <= 64, digests)."""
+    z = H.gold("lll_ranged_ref.npz")
+    p = "c%d_" % case
+    ops = json.loads(bytes(z[p + "ops_json"]).decode())
+    m = O.OracleGSO(z[p + "b"].astype(np.int64))
+    t = 0
+    for op in ops:
+        r = H.ranged_apply(m, op)
+        if r is None:
+            continue
+        got = [int(r["ok"]), r["status"]] + ([r["n_swaps"], r["final_kappa"], r["zeros"]] if op[0] == "lll" else [])
+        assert got == list(z[p + "res"][t][: len(got)]), "call %d %s" % (t, op)
+        s = m.state()
+        if p + "s_mu" in z:
+            ref = {k: z[p + "s_" + k][t] for k in ["n_known_rows", "n_known_cols", "n_source_rows", "row_expo",
+                                                  "gso_valid_cols", "init_row_size", "b", "bf", "gf", "mu", "r"]}
+            ref["b"] = ref["b"].astype(np.int64)
+            H.assert_state_equal(s, ref, "call %d %s" % (t, op))
+        assert H.gso_digest(s) == z[p + "digest"][t], "call %d %s digest" % (t, op)
+        t += 1
+    assert t == len(z[p + "res"])
+    if p + "b_out" in z:
+        assert np.array_equal(m.state()["b"], z[p + "b_out"])

@@ -94,44 +94,17 @@ def test_device_lll_vs_reference_size_fixture(fb, lll_mode, tag):
 
 def test_ranged_lll_and_size_reduction_resume_d300(fb, lll_mode):
     """lll(0,0,k) / size_reduction(0,k) with prefixes ending on both sides of row 256 and a row above it touched in
-    between: the basis must equal a from-scratch oracle run of the same call sequence."""
-    import ctypes as C
-    from fplll_b200.gso import _lib, _ck, _ptr
+    between: status, n_swaps, zeros, final_kappa and the whole state after every call must equal the ranged oracle's on
+    the same continuing object."""
+    from test_lll_ranged_gpu import Pair
     rng = np.random.default_rng(42)
     d = 300
-    b = rng.integers(-(1 << 12), 1 << 12, size=(d, d), dtype=np.int64)
-    md = fb.MatGSO(b)
-    st = np.zeros(1, np.int32)
-
-    def dev_lll(kend):
-        _ck(_lib().b200gso_lll_range(md._h, 0.99, 0.51, 0, 0, kend, 0, _ptr(st, C.c_int), None), "lll_range")
-        return int(st[0])
-
-    def dev_sr(kend):
-        _ck(_lib().b200gso_size_reduction(md._h, 0.51, 0, kend, 0, _ptr(st, C.c_int)), "size_reduction")
-        return int(st[0])
-
-    def ora_lll(bb, kend):
-        # lll(0, 0, kend) of the reference on the rows < kend: a fresh oracle on those rows
-        sub = O.OracleGSO(bb[:kend])
-        r = sub.lll(0.99, 0.51)
-        out = bb.copy()
-        out[:kend] = sub.state()["b"]
-        return r["status"], out
-    bb = b
-    for kend in (240, 280):
-        assert dev_lll(kend) == 0
-        s, bb = ora_lll(bb, kend)
-        assert s == 0 and np.array_equal(md.b[0], bb), "lll(0, 0, %d)" % kend
-    md.row_addmul_we(262, 3, 7.0, 0)
-    md.row_op_end(262, 263)
-    mo = O.OracleGSO(bb)
-    mo.row_addmul_we(262, 3, 7.0, 0)
-    mo.row_op_end(262, 263)
-    assert dev_sr(290) == 0
-    assert dev_lll(300) == 0
-    s, bb = ora_lll(mo.state()["b"], 300)
-    assert s == 0 and np.array_equal(md.b[0], bb)
+    p = Pair(fb, rng.integers(-(1 << 12), 1 << 12, size=(1, d, d), dtype=np.int64))
+    p.lll(kend=240)
+    p.lll(kend=280)
+    p.run([["addmul", 262, 3, 7.0]])
+    p.sr(kend=290)
+    p.lll(kend=300)
 
 
 @pytest.mark.parametrize("flags", [2, 0])
