@@ -6,7 +6,8 @@ Host-side mirror of the reference classes (same method names, argument meaning a
 All compute happens in hand-written sm_90a kernels behind the C-ABI of include/*.h.
 """
 from ._lib import B200Error  # noqa: F401
-from .gso import MatGSO, lll_reduction, GSO_DEFAULT, GSO_ROW_EXPO, GSO_OP_FORCE_LONG  # noqa: F401
+from .gso import MatGSO, lll_reduction, GSO_DEFAULT, GSO_ROW_EXPO, GSO_OP_FORCE_LONG, GSO_TRANSFORM  # noqa: F401
+from .gso import OP_ROW_ADDMUL, OP_MOVE_ROW, OP_ROW_SWAP, OP_ROW_OP_END, OP_NEGATE  # noqa: F401
 from .gso import RED_SUCCESS, RED_GSO_FAILURE, RED_BABAI_FAILURE, RED_LLL_FAILURE  # noqa: F401
 from .bkz import BKZParam, bkz_reduction, load_strategies  # noqa: F401
 from .bkz import BKZ_DEFAULT, BKZ_VERBOSE, BKZ_NO_LLL, BKZ_MAX_LOOPS, BKZ_AUTO_ABORT, BKZ_GH_BND, BKZ_SHRINK_RADIUS  # noqa: F401

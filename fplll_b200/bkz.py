@@ -49,6 +49,8 @@ def _lib():
         L.b200bkz_add_strategy.argtypes = [C.c_void_p, C.c_int, _P(C.c_int), C.c_int, _P(C.c_double), _P(C.c_double),
                                            _P(C.c_double), C.c_int]
         L.b200bkz_reduce.argtypes = [C.c_void_p, C.c_int, C.c_int, _P(C.c_int64), _P(_Param), _P(_Stats)]
+        L.b200bkz_reduce_transform.argtypes = [C.c_void_p, C.c_int, C.c_int, _P(C.c_int64), _P(C.c_int64),
+                                               _P(_Param), _P(_Stats)]
         _done = True
     return L
 
@@ -73,10 +75,12 @@ class BKZParam:
         self.rerandomization_density, self.seed = rerandomization_density, seed
 
 
-def bkz_reduction(b, param, devices=None):
+def bkz_reduction(b, param, devices=None, u=None):
     """bkz_reduction(ZZ_mat<long>& b, BKZParam) in the int64 regime (bkz.cpp:812-836): reduces the (d, n) int64 numpy
     array IN PLACE.  BKZ 2.0 by default, self-dual BKZ with BKZ_SD_VARIANT, slide reduction with BKZ_SLD_RED.  Returns (RedStatus, stats dict).  param.strategies: None (EmptyStrategy for every block size),
-    "default" (the reference's strategies/default.json table) or a dict as returned by load_strategies."""
+    "default" (the reference's strategies/default.json table) or a dict as returned by load_strategies.
+    u: a (d, d) int64 array overwritten with the transform of the whole call, U * b_in == b_out (bkz_reduction(b, u,
+    param), which starts u at the identity, bkz.cpp:857-859); b, status and stats are those of the call without u."""
     L = _lib()
     arr = np.ascontiguousarray(b, dtype=np.int64)
     d, n = arr.shape
@@ -103,10 +107,17 @@ def bkz_reduction(b, param, devices=None):
         p.gh_factor, p.min_success_probability = param.gh_factor, param.min_success_probability
         p.rerandomization_density, p.seed = param.rerandomization_density, param.seed
         st = _Stats()
-        rc = L.b200bkz_reduce(h, d, n, arr.ctypes.data_as(_P(C.c_int64)), C.byref(p), C.byref(st))
+        if u is None:
+            rc = L.b200bkz_reduce(h, d, n, arr.ctypes.data_as(_P(C.c_int64)), C.byref(p), C.byref(st))
+        else:
+            ua = np.eye(d, dtype=np.int64)
+            rc = L.b200bkz_reduce_transform(h, d, n, arr.ctypes.data_as(_P(C.c_int64)), ua.ctypes.data_as(_P(C.c_int64)),
+                                            C.byref(p), C.byref(st))
         if rc:
             raise B200Error("b200bkz_reduce failed (%d): %s" % (rc, L.b200bkz_last_error().decode()))
     finally:
         L.b200bkz_destroy(h)
     b[...] = arr
+    if u is not None:
+        u[...] = ua
     return st.status, {f: getattr(st, f) for f, _ in _Stats._fields_}

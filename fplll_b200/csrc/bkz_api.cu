@@ -765,7 +765,12 @@ int b200bkz_add_strategy(b200bkz_t *h, int block_size, const int *preproc, int n
   return 0;
 }
 
-int b200bkz_reduce(b200bkz_t *h, int d, int n, int64_t *b, const b200bkz_param *param, b200bkz_stats *stats)
+}  // extern "C"
+
+// b200bkz_reduce (u == nullptr) and b200bkz_reduce_transform: u rides along on a B200GSO_TRANSFORM handle, which takes
+// every decision exactly as an untransformed one would.
+static int bkz_reduce(b200bkz_t *h, int d, int n, int64_t *b, int64_t *u, const b200bkz_param *param,
+                      b200bkz_stats *stats)
 {
   if (!h || !b || !param || d < 1 || n < 1)
   {
@@ -782,7 +787,7 @@ int b200bkz_reduce(b200bkz_t *h, int d, int n, int64_t *b, const b200bkz_param *
     stats = &local;
   memset(stats, 0, sizeof(*stats));
   b200gso_t *g = nullptr;
-  int rc       = b200gso_create(&g, 1, d, n, B200GSO_ROW_EXPO, h->devs[0]);  // bkz.cpp:819-820
+  int rc       = b200gso_create(&g, 1, d, n, B200GSO_ROW_EXPO | (u ? B200GSO_TRANSFORM : 0), h->devs[0]);  // bkz.cpp:819-820
   if (rc)
   {
     g_bkz_err = b200gso_last_error();
@@ -793,6 +798,8 @@ int b200bkz_reduce(b200bkz_t *h, int d, int n, int64_t *b, const b200bkz_param *
   try
   {
     GCK(b200gso_set_basis(g, b));
+    if (u)
+      GCK(b200gso_set_transform(g, u));  // the caller's U (bkz.cpp:857-859 starts it at the identity)
     Driver drv(h, g, d, *param, stats);
     double tb = now_s();
     try
@@ -859,6 +866,8 @@ int b200bkz_reduce(b200bkz_t *h, int d, int n, int64_t *b, const b200bkz_param *
       stats->r00_after = ldexp(m, (int)e);
     }
     GCK(b200gso_get_basis(g, b));
+    if (u)
+      GCK(b200gso_get_transform(g, u));
   }
   catch (std::exception &ex)
   {
@@ -873,6 +882,24 @@ int b200bkz_reduce(b200bkz_t *h, int d, int n, int64_t *b, const b200bkz_param *
   (void)t0;
   b200gso_destroy(g);
   return ret;
+}
+
+extern "C" {
+
+int b200bkz_reduce(b200bkz_t *h, int d, int n, int64_t *b, const b200bkz_param *param, b200bkz_stats *stats)
+{
+  return bkz_reduce(h, d, n, b, nullptr, param, stats);
+}
+
+int b200bkz_reduce_transform(b200bkz_t *h, int d, int n, int64_t *b, int64_t *u, const b200bkz_param *param,
+                             b200bkz_stats *stats)
+{
+  if (!u)
+  {
+    g_bkz_err = "b200bkz_reduce_transform: u is NULL";
+    return B200BKZ_EINVAL;
+  }
+  return bkz_reduce(h, d, n, b, u, param, stats);
 }
 
 }  // extern "C"

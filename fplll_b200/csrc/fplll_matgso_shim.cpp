@@ -30,8 +30,12 @@
 // On top of that, BKZReduction<Z_NR<long>, FP_NR<double>>::bkz() (bkz.cpp:522-672) — what bkz_reduction() / `fplll -a bkz`
 // run after their wrapper-LLL when the basis fits long (bkz.cpp:812-836) — is taken over whole by the device driver
 // (b200bkz_reduce: device-resident LLL loops, device enumeration, no per-call forwarding) whenever the request is one
-// that driver implements: BKZ 2.0, SD-BKZ (-a sdb) and slide reduction (-a sld), without transformation matrices or a GSO
-// dump.  Both SD and slide flags together go to the reference, which throws its own error.  B200_SHIM_BKZ=0 turns the
+// that driver implements: BKZ 2.0, SD-BKZ (-a sdb) and slide reduction (-a sld), without a GSO dump, with or without the
+// transform u (`fplll -a bkz -of bu`: mg->u travels through b200bkz_reduce_transform and is written back; the one
+// difference from the reference's u is that a row of b negated by svp_postprocessing negates the row of u too, so the
+// returned u always satisfies u * B_in = B_out — B200GSO_TRANSFORM in b200gso.h), but never with u_inv_t
+// (enable_inverse_transform: that stays with the reference).  Both SD and slide flags together go to the reference,
+// which throws its own error.  B200_SHIM_BKZ=0 turns the
 // take-over off (every algorithm then runs the reference's control flow over the forwarded GSO).
 //
 // Build (where fplll's headers are installed):  g++ -shared -fPIC fplll_matgso_shim.cpp -lb200bkz -ldl  -> libb200fplll.so
@@ -396,13 +400,15 @@ template <> bool BKZReduction<Z_NR<long>, FP_NR<double>>::bkz()
   static const bool takeover = b200shim::enabled() && !(getenv("B200_SHIM_BKZ") && atoi(getenv("B200_SHIM_BKZ")) == 0);
   auto *mg = dynamic_cast<MatGSO<Z_NR<long>, FP_NR<double>> *>(&m);
   const bool sd_and_sld = (param.flags & BKZ_SD_VARIANT) && (param.flags & BKZ_SLD_RED);
-  if (!takeover || !mg || (param.flags & BKZ_DUMP_GSO) || sd_and_sld || mg->enable_int_gram || mg->enable_transform ||
-      param.block_size < 2 || num_rows != mg->b.get_rows() || num_rows > 512 || b200gso_device_count() == 0)
+  const int d = mg ? mg->b.get_rows() : 0, n = mg ? mg->b.get_cols() : 0;
+  const bool xf = mg && mg->enable_transform;
+  if (!takeover || !mg || (param.flags & BKZ_DUMP_GSO) || sd_and_sld || mg->enable_int_gram ||
+      mg->enable_inverse_transform || (xf && (mg->u.get_rows() != d || mg->u.get_cols() != d)) ||
+      param.block_size < 2 || num_rows != d || num_rows > 512 || b200gso_device_count() == 0)
     return orig(this);
   // what the reference's bkz() sets first (bkz.cpp:527-529): set_status prints it under BKZ_VERBOSE, and a null char*
   // written to cerr would silence the caller's cerr for good
   algorithm   = (param.flags & BKZ_SD_VARIANT) ? "SD-BKZ" : (param.flags & BKZ_SLD_RED) ? "SLD" : "BKZ";
-  const int d = mg->b.get_rows(), n = mg->b.get_cols();
   b200bkz_t *h = nullptr;
   int dev0     = 0;
   if (b200bkz_create(&h, &dev0, 1) != 0)
@@ -437,8 +443,13 @@ template <> bool BKZReduction<Z_NR<long>, FP_NR<double>>::bkz()
   for (int i = 0; i < d; i++)
     for (int j = 0; j < n; j++)
       flat[(size_t)i * n + j] = mg->b(i, j).get_si();
+  std::vector<int64_t> uflat(xf ? (size_t)d * d : 0);
+  for (int i = 0; i < (xf ? d : 0); i++)
+    for (int j = 0; j < d; j++)
+      uflat[(size_t)i * d + j] = mg->u(i, j).get_si();
   b200bkz_stats stt;
-  const int rc = b200bkz_reduce(h, d, n, flat.data(), &p, &stt);
+  const int rc = xf ? b200bkz_reduce_transform(h, d, n, flat.data(), uflat.data(), &p, &stt)
+                    : b200bkz_reduce(h, d, n, flat.data(), &p, &stt);
   b200bkz_destroy(h);
   if (rc != 0)
     throw std::runtime_error(std::string("b200 shim: b200bkz_reduce: ") + b200bkz_last_error());
@@ -447,6 +458,9 @@ template <> bool BKZReduction<Z_NR<long>, FP_NR<double>>::bkz()
   for (int i = 0; i < d; i++)
     for (int j = 0; j < n; j++)
       mg->b(i, j) = (long)flat[(size_t)i * n + j];
+  for (int i = 0; i < (xf ? d : 0); i++)
+    for (int j = 0; j < d; j++)
+      mg->u(i, j) = (long)uflat[(size_t)i * d + j];
   m.row_op_end(0, d);
   nodes = (long)stt.enum_nodes;
   g_bkz_taken++;

@@ -194,6 +194,8 @@ __global__ void k_move_row(Batch S, int old_r, int new_r)
   if (!warp_setup(S, v, s, lov, lane))
     return;
   warp_move_row(v, old_r, new_r, lane);
+  if (v.u && old_r != new_r)
+    warp_move_u_row(v, old_r, new_r, lane);
 }
 
 __global__ void k_set_r(Batch S, int i, int j, const double *f)
@@ -302,21 +304,21 @@ __global__ void k_apply_ops(Batch S, const b200gso_op *ops, int n)
     switch (op.type)
     {
     case B200GSO_OP_ROW_ADDMUL: warp_row_addmul_we(v, op.a, op.b, op.x, 0, lane); break;
-    case B200GSO_OP_MOVE_ROW: warp_move_row(v, op.a, op.b, lane); break;
+    case B200GSO_OP_MOVE_ROW:
+      warp_move_row(v, op.a, op.b, lane);
+      if (v.u && op.a != op.b)
+        warp_move_u_row(v, op.a, op.b, lane);
+      break;
     case B200GSO_OP_ROW_SWAP: warp_row_swap(v, op.a, op.b, lane); break;
     case B200GSO_OP_ROW_OP_END: warp_row_op_end(v, op.a, op.b, lane); break;
-    case B200GSO_OP_NEGATE:
-      lower_clean(v, op.a, lane);
-      for (int c = lane; c < v.n; c += 32)
-        v.b[(size_t)op.a * v.ldb + c] = -v.b[(size_t)op.a * v.ldb + c];
-      break;
+    case B200GSO_OP_NEGATE: warp_negate_row(v, op.a, lane); break;
     }
     __syncwarp();
   }
   mc.store(v, lane);
 }
 
-// MatGSO::negate_row_of_b(i), gso.h:291-297 (integer row only)
+// MatGSO::negate_row_of_b(i), gso.h:291-297 (integer row only), and row i of U on a transform handle (warp_negate_row)
 __global__ void k_negate_row(Batch S, int i)
 {
   const int l = blockIdx.y;
@@ -328,6 +330,17 @@ __global__ void k_negate_row(Batch S, int i)
   }
   for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < S.n; c += gridDim.x * blockDim.x)
     v.b[(size_t)i * S.ldb + c] = -v.b[(size_t)i * S.ldb + c];
+  if (v.u)
+    for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < S.d; c += gridDim.x * blockDim.x)
+      u_row(v, i)[c] = -u_row(v, i)[c];
+}
+
+// U = identity on every lattice (the buffer was zeroed)
+__global__ void k_u_identity(Batch S)
+{
+  View v = S.view(blockIdx.x);
+  for (int i = threadIdx.x; i < S.d; i += blockDim.x)
+    u_row(v, i)[i] = 1;
 }
 
 __global__ void k_get_r_diag(Batch S, int l, int first, int count, double *rmant, long *rexpo)
@@ -404,9 +417,15 @@ int b200gso_device_count(void)
 
 int b200gso_create(b200gso_t **out, int batch, int d, int n, int flags, int device)
 {
-  if (!out || batch <= 0 || d <= 0 || n <= 0 || (flags & 1) || (flags & ~(1 | 2 | 4 | B200GSO_HOST_BASIS)))
+  if (!out || batch <= 0 || d <= 0 || n <= 0 || (flags & 1) ||
+      (flags & ~(1 | 2 | 4 | B200GSO_HOST_BASIS | B200GSO_TRANSFORM)))
   {
     g_err = "b200gso_create: bad arguments (GSO_INT_GRAM is not supported on the device)";
+    return B200GSO_EINVAL;
+  }
+  if ((flags & B200GSO_TRANSFORM) && (flags & B200GSO_HOST_BASIS))
+  {
+    g_err = "b200gso_create: B200GSO_TRANSFORM needs the int64 basis on the device (not B200GSO_HOST_BASIS)";
     return B200GSO_EINVAL;
   }
   if (b200gso_device_count() <= device)
@@ -430,7 +449,11 @@ int b200gso_create(b200gso_t **out, int batch, int d, int n, int flags, int devi
   S.mu_stride      = mu_size(d);
   S.tri_stride     = tri_size(d);
   S.scratch_stride = tri_size(d);
+  S.u              = nullptr;
+  S.u_stride       = (flags & B200GSO_TRANSFORM) ? (size_t)d * ld_b(d) : 0;
   int rc = 0;
+  if (flags & B200GSO_TRANSFORM)
+    rc |= dev_alloc(h, &S.u, S.u_stride * batch);
   rc |= dev_alloc(h, &S.b, S.b_stride * batch);
   rc |= dev_alloc(h, &S.bf, S.bf_stride * batch);
   rc |= dev_alloc(h, &S.mu, S.mu_stride * batch);
@@ -510,6 +533,15 @@ int b200gso_create(b200gso_t **out, int batch, int d, int n, int flags, int devi
   if (me == cudaSuccess) me = cudaMemsetAsync(S.r, 0, S.tri_stride * batch * sizeof(double), h->stream);
   if (me == cudaSuccess) me = cudaMemsetAsync(S.gf, 0, S.tri_stride * batch * sizeof(double), h->stream);
   if (me == cudaSuccess) me = cudaMemsetAsync(S.meta, 0, (size_t)M_STRIDE * batch * sizeof(int), h->stream);
+  if (me == cudaSuccess && S.u)
+  {
+    me = cudaMemsetAsync(S.u, 0, S.u_stride * batch * sizeof(int64_t), h->stream);
+    if (me == cudaSuccess)
+    {
+      k_u_identity<<<batch, 128, 0, h->stream>>>(S);
+      me = cudaGetLastError();
+    }
+  }
   if (me == cudaSuccess) me = cudaStreamSynchronize(h->stream);
   if (me != cudaSuccess)
   {
@@ -632,11 +664,43 @@ int b200gso_upload_row_fp(b200gso_t *h, int i, const double *bf_rows, const long
   return 0;
 }
 
+// U (batch x d x d, dense) <-> the device's ld_b(d)-strided rows: one 2D copy, every lattice's rows share the pitch
+static int copy_transform(b200gso_t *h, int64_t *dst, const int64_t *src, bool to_device)
+{
+  if (!h || (to_device ? !src : !dst))
+    return B200GSO_EINVAL;
+  if (!h->S.u)
+  {
+    g_err = "b200gso_set/get_transform: the handle was created without B200GSO_TRANSFORM";
+    return B200GSO_EINVAL;
+  }
+  CK(cudaSetDevice(h->device));
+  const size_t d = h->S.d, dev_pitch = ld_b(h->S.d) * sizeof(int64_t), rows = (size_t)h->S.B * d;
+  if (to_device)
+    CK(cudaMemcpy2DAsync(h->S.u, dev_pitch, src, d * sizeof(int64_t), d * sizeof(int64_t), rows,
+                         cudaMemcpyHostToDevice, h->stream));
+  else
+    CK(cudaMemcpy2DAsync(dst, d * sizeof(int64_t), h->S.u, dev_pitch, d * sizeof(int64_t), rows,
+                         cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  CK(cudaGetLastError());
+  return 0;
+}
+
+int b200gso_set_transform(b200gso_t *h, const int64_t *u) { return copy_transform(h, nullptr, u, true); }
+
+int b200gso_get_transform(b200gso_t *h, int64_t *u) { return copy_transform(h, u, nullptr, false); }
+
 int b200gso_upload_row(b200gso_t *h, int i, const int64_t *rows)
 {
   if (!h || !rows || i < 0 || i >= h->S.d)
     return B200GSO_EINVAL;
   NO_HOST_BASIS(h);
+  if (h->S.u)
+  {
+    g_err = "b200gso_upload_row: a row rewritten on the host leaves U unknown (handle is B200GSO_TRANSFORM)";
+    return B200GSO_EINVAL;
+  }
   CK(cudaSetDevice(h->device));
   // stream-ordered: with pinned `rows` this returns without waiting (the caller must not reuse `rows` before the
   // next synchronising call); pageable memory makes cudaMemcpyAsync stage synchronously, which is also correct.

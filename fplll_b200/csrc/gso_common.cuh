@@ -45,7 +45,7 @@ struct MetaCache
   int *g_valid, *g_expo, *g_irs, *g_meta;
   int d;
   __host__ __device__ static size_t ints(int d) { return 3 * (size_t)((d + 3) & ~3) + M_STRIDE; }
-  __device__ void load(View &v, int *sm, int lane)
+  __device__ void load(ViewCore &v, int *sm, int lane)
   {
     d = v.d;
     const int dp = (d + 3) & ~3;
@@ -62,7 +62,7 @@ struct MetaCache
     v.valid = s_valid, v.row_expo = s_expo, v.irs = s_irs, v.meta = s_meta;
     __syncwarp();
   }
-  __device__ void store(const View &v, int lane)
+  __device__ void store(const ViewCore &v, int lane)
   {
     __syncwarp();
     for (int i = lane; i < d; i += 32)

@@ -21,6 +21,7 @@
 // flow).  No spin-waits.
 #pragma once
 #include "gso_warp.cuh"
+#include <type_traits>
 
 namespace b200 {
 
@@ -64,6 +65,10 @@ static __device__ long long g_cta_prof[32];
 #define CTA_PCNT_IF(cond, slot, val)
 #endif
 
+// The view the LLL loops carry: the full View when the kernel tracks U, else ViewCore — the one-CTA kernel keeps the
+// master's view in its stack frame, and a larger struct there would change the untransformed kernels' code.
+template <bool XF> using LLLView = typename std::conditional<XF, View, ViewCore>::type;
+
 constexpr int CTA_WARPS = 8;
 constexpr int CTA_OWN   = 2;  // panels a warp can own: 16 panels = d <= 512
 
@@ -71,7 +76,7 @@ enum { COOP_EXIT = 0, COOP_UPDATE = 1, COOP_BACKSUB = 2, COOP_IGEMV = 3, COOP_MU
 
 struct CoopShared
 {
-  View v;      // the master's view (its metadata pointers point into the master's shared-memory cache)
+  ViewCore v;  // the master's view (its metadata pointers point into the master's shared-memory cache)
   WarpSmem s;  // the master's scratch rows (vb, rrow, murow, aux, xs)
   double *bm;  // babai_mu row handed to BACKSUB
   // Shared-memory cache of the leading mu panels, as many as fit next to the rest of the CTA's shared memory (none at
@@ -92,6 +97,7 @@ struct CoopShared
   double epoch;
   int cmd, a0, a1, a2;
   int flag;
+  int64_t *u;  // the master's U (transform kernels only, row stride ld_b(d)); last, so that no other member moves
 };
 
 __device__ inline void pub_store(double *slot, double val, double tag)
@@ -238,7 +244,7 @@ __device__ inline double lane_dot_deep(const double *__restrict__ col, const dou
 // (products in parallel, one ordered subtraction chain) when it is asked for, then gso_valid_cols[i].
 __device__ inline bool cta_update_diag(CoopShared &C, int i, int last_j, int j0, int ncols, int tid)
 {
-  const View v     = C.v;  // by value: registers, not a reload from shared memory after every store
+  const ViewCore v = C.v;  // by value: registers, not a reload from shared memory after every store
   const WarpSmem s = C.s;
   double *gfrow = v.gf + tri_off(i), *rrow_g = v.r + tri_off(i);
   CTA_PT(tp2_);
@@ -280,7 +286,7 @@ __device__ inline bool cta_update_diag(CoopShared &C, int i, int last_j, int j0,
 //   acc_j = g(i,j); acc_j -= mu(j,k) r(i,k) for k = 0 .. j-1 ascending.
 __device__ inline bool cta_update_gso_row(CoopShared &C, int i, int last_j, int w, int lane)
 {
-  const View v     = C.v;  // by value: registers, not a reload from shared memory after every store
+  const ViewCore v = C.v;  // by value: registers, not a reload from shared memory after every store
   const WarpSmem s = C.s;
   const int tid = threadIdx.x;
   const int j0  = max(0, v.valid[i]);
@@ -517,7 +523,7 @@ __device__ inline bool cta_update_gso_row(CoopShared &C, int i, int last_j, int 
 // babai_mu (columns < sr_end); the X_j land in s.xs[j], the per-panel masks of the non-zero ones in xmask[].
 __device__ inline void cta_backsub(CoopShared &C, int kappa, int sr_end, int sr_start, int w, int lane)
 {
-  const View v     = C.v;  // by value: registers, not a reload from shared memory after every store
+  const ViewCore v = C.v;  // by value: registers, not a reload from shared memory after every store
   const WarpSmem s = C.s;
   const int ek  = v.row_expo[kappa];
   unsigned *xmask = (unsigned *)(s.xs + ((v.d + 1) & ~1));
@@ -692,20 +698,25 @@ __device__ inline void cta_backsub(CoopShared &C, int kappa, int sr_end, int sr_
 // ---- IGEMV ----------------------------------------------------------------------------------------------------------
 // b_kappa += sum_t lx_t * 2^e_t * b_{row_t} over the nnz compacted rows (lx in s.aux[t], (e << 32 | row) in s.murow[t]):
 // row_addmul_we (gso.cpp:236-262) fused over j; int64 arithmetic wraps, so the order of the additions is immaterial.
-// Warp w takes the column groups w, w + CTA_WARPS, ... of 32 columns.
+// Warp w takes the column groups w, w + CTA_WARPS, ... of 32 columns.  XF (transform): the column space is b's nc
+// columns followed by the d columns of U, column c >= nc being U's column c - nc — one pass over both.
+template <bool XF>
 __device__ inline void cta_igemv(CoopShared &C, int kappa, int nnz, int w, int lane)
 {
-  const View v     = C.v;  // by value: registers, not a reload from shared memory after every store
+  const ViewCore v = C.v;  // by value: registers, not a reload from shared memory after every store
   const WarpSmem s = C.s;
   const int nc  = v.meta[M_NKC];
   CTA_PT(ti0_);
   CTA_PCNT(9, 1);
   CTA_PCNT(10, nnz);
+  const int ncx = XF ? nc + v.d : nc;
+  const size_t ldu = ld_b(v.d);
   unsigned long long *bk = (unsigned long long *)(v.b + (size_t)kappa * v.ldb);
-  for (int c0 = 32 * w; c0 < nc; c0 += 32 * CTA_WARPS)
+  unsigned long long *uk = XF ? (unsigned long long *)(C.u + (size_t)kappa * ldu) : nullptr;
+  for (int c0 = 32 * w; c0 < ncx; c0 += 32 * CTA_WARPS)
   {
     const int c = c0 + lane;
-    unsigned long long acc = (c < nc) ? bk[c] : 0ull;
+    unsigned long long acc = (c < nc) ? bk[c] : (XF && c < ncx) ? uk[c - nc] : 0ull;
     for (int t0 = 0; t0 < nnz; t0 += 16)
     {
       unsigned long long bv[16], lxv[16];
@@ -723,6 +734,8 @@ __device__ inline void cta_igemv(CoopShared &C, int kappa, int nnz, int w, int l
           const unsigned long long *src = (const unsigned long long *)(v.b + (size_t)(int)(pk & 0xffffffffll) * v.ldb);
           if (c < nc)
             bv[x] = src[c];
+          else if (XF && c < ncx)
+            bv[x] = ((const unsigned long long *)(C.u + (size_t)(int)(pk & 0xffffffffll) * ldu))[c - nc];
         }
       }
 #pragma unroll
@@ -734,6 +747,8 @@ __device__ inline void cta_igemv(CoopShared &C, int kappa, int nnz, int w, int l
     }
     if (c < nc)
       bk[c] = acc;
+    else if (XF && c < ncx)
+      uk[c - nc] = acc;
   }
   cta_bar(2);
   CTA_PADD(11, ti0_);
@@ -779,10 +794,11 @@ __device__ inline void cta_mu_load(CoopShared &C, int pa, int pb, int w, int lan
 // ---- MOVE -----------------------------------------------------------------------------------------------------------
 // move_row(old_r, new_r) (gso.cpp:289-366) by the whole CTA: warp_move_row (gso_warp.cuh) with its lane-strided passes
 // (one column of mu / r / b / bf per lane, one Gram row per lane) strided over all CTA_WARPS * 32 threads instead; the
-// data movement per element is the same, only who carries it differs.
+// data movement per element is the same, only who carries it differs.  XF: the rows of U rotate with those of b.
+template <bool XF>
 __device__ inline void cta_move_row(CoopShared &C, int old_r, int new_r, int w, int lane)
 {
-  const View v  = C.v;
+  const ViewCore v = C.v;
   const int tid = threadIdx.x, NT = CTA_WARPS * 32;
   if (old_r == new_r)
   {
@@ -809,6 +825,13 @@ __device__ inline void cta_move_row(CoopShared &C, int old_r, int new_r, int w, 
   {
     rotate_seq<int64_t>([&](int i) -> int64_t & { return v.b[(size_t)i * v.ldb + c]; }, lo, hi, right);
     rotate_seq<double>([&](int i) -> double & { return v.bf[bf_off(i, c, v.n)]; }, lo, hi, right);
+  }
+  if (XF)
+  {
+    int64_t *const u = C.u;
+    const size_t ldu = ld_b(v.d);
+    for (int c = tid; c < v.d; c += NT)
+      rotate_seq<int64_t>([&](int i) -> int64_t & { return u[(size_t)i * ldu + c]; }, lo, hi, right);
   }
   const int ghi      = right ? hi : min(hi, nkr - 1);
   const bool do_gram = right || lo < nkr - 1;
@@ -862,6 +885,7 @@ __device__ inline void cta_move_row(CoopShared &C, int old_r, int new_r, int w, 
 }
 
 // helper warps: wait for commands until the master says EXIT
+template <bool XF>
 __device__ inline void coop_helper_loop(CoopShared &C, int w, int lane)
 {
   for (;;)
@@ -875,17 +899,17 @@ __device__ inline void coop_helper_loop(CoopShared &C, int w, int lane)
     else if (cmd == COOP_BACKSUB)
       cta_backsub(C, a0, a1, a2, w, lane);
     else if (cmd == COOP_IGEMV)
-      cta_igemv(C, a0, a1, w, lane);
+      cta_igemv<XF>(C, a0, a1, w, lane);
     else if (cmd == COOP_MULOAD)
       cta_mu_load(C, a0, a1, w, lane);
     else if (cmd == COOP_MOVE)
-      cta_move_row(C, a0, a1, w, lane);
+      cta_move_row<XF>(C, a0, a1, w, lane);
   }
 }
 
 // master side of update_gso_row: the reference's early exits, then the cooperative operation
 template <bool COOP>
-__device__ inline bool lll_update_gso_row(const View &v, int i, int last_j, WarpSmem &s, int lane, CoopShared *C)
+__device__ inline bool lll_update_gso_row(const ViewCore &v, int i, int last_j, WarpSmem &s, int lane, CoopShared *C)
 {
   if (!COOP)
     return warp_update_gso_row(v, i, last_j, s, lane);
@@ -912,7 +936,7 @@ __device__ inline bool lll_update_gso_row(const View &v, int i, int last_j, Warp
 }
 
 // mu(i,k) as the LLL loop reads it: the one-CTA kernel through its cached panels
-template <bool COOP> __device__ inline double lll_mu_load(const View &v, const CoopShared *C, int i, int k)
+template <bool COOP> __device__ inline double lll_mu_load(const ViewCore &v, const CoopShared *C, int i, int k)
 {
   return COOP ? coop_mu_load(*C, i, k) : v.mu[mu_off(i, k)];
 }
@@ -936,15 +960,19 @@ template <bool COOP> __device__ inline void lll_mu_refresh_diag(CoopShared *C, i
   __syncwarp();
 }
 
-template <bool COOP> __device__ inline void lll_move_row(const View &v, int old_r, int new_r, int lane, CoopShared *C)
+template <bool COOP, bool XF>
+__device__ inline void lll_move_row(const LLLView<XF> &v, int old_r, int new_r, int lane, CoopShared *C)
 {
   if (!COOP)
   {
     warp_move_row(v, old_r, new_r, lane);
+    if constexpr (XF)
+      if (old_r != new_r)
+        warp_move_u_row(v, old_r, new_r, lane);
     return;
   }
   coop_post(C, COOP_MOVE, old_r, new_r, 0, lane);
-  cta_move_row(*C, old_r, new_r, 0, lane);
+  cta_move_row<XF>(*C, old_r, new_r, 0, lane);
 }
 
 }  // namespace b200

@@ -23,6 +23,8 @@
 //           starts 16-byte aligned: row i starts at ((i+1)^2)>>1 and holds i+1 (+pad) doubles.  These are only
 //           ever touched as whole rows (read r(i,0..), write r(i,.), gf(i,.)), which row-packed makes coalesced.
 //   b   : int64, row-major, row stride ldb = n rounded up to even (16-byte aligned rows for 128-bit row ops).
+//   u   : int64, row-major d x d, row stride ld_b(d) — the transform U of a B200GSO_TRANSFORM handle (null otherwise).
+//         Every integer row operation on b is applied to the row of u with the same index, over all d columns.
 //
 // NaN in gf marks an invalid Gram entry exactly as in the reference (gso.cpp:50-54, gso.h:324).
 #pragma once
@@ -53,8 +55,10 @@ enum
   M_DELTA_LO = 6, M_DELTA_HI = 7, M_ETA_LO = 8, M_ETA_HI = 9, M_STRIDE = 16
 };
 
-// One lattice's state (device pointers).
-struct View
+// One lattice's state (device pointers) without the transform.  The CTA LLL keeps a copy of it in shared memory
+// (CoopShared, gso_cta.cuh) and carries u next to it, so that adding u changed neither that layout nor the code of the
+// kernels that never touch u.
+struct ViewCore
 {
   int d, n, ldb, row_expo_en;
   int host_basis;  // B200GSO_HOST_BASIS: b is not on the device, bf rows are uploaded by the host
@@ -62,6 +66,10 @@ struct View
   double *bf, *mu, *r, *gf;
   int *row_expo, *valid, *irs, *meta;
   double *scratch;  // >= tri_size(d) + 2*d*ld + ... doubles, see gso_api
+};
+struct View : ViewCore
+{
+  int64_t *u;  // B200GSO_TRANSFORM: d x d, row stride ld_b(d); nullptr otherwise
 };
 
 // A batch: base pointers + per-lattice strides.
@@ -73,6 +81,8 @@ struct Batch
   double *bf, *mu, *r, *gf, *scratch;
   int *row_expo, *valid, *irs, *meta;
   size_t b_stride, bf_stride, mu_stride, tri_stride, scratch_stride;
+  int64_t *u;  // B200GSO_TRANSFORM handles only (nullptr otherwise), u_stride = d * ld_b(d) per lattice
+  size_t u_stride;
 
   __host__ __device__ View view(int l) const
   {
@@ -88,6 +98,7 @@ struct Batch
     v.valid    = valid + (size_t)l * d;
     v.irs      = irs + (size_t)l * d;
     v.meta     = meta + (size_t)l * M_STRIDE;
+    v.u        = u ? u + (size_t)l * u_stride : nullptr;
     return v;
   }
 };

@@ -36,9 +36,10 @@ struct LLLStats
 #endif
 
 // LLLReduction::babai(kappa, size_reduction_end, size_reduction_start), lll.cpp:166-224.
-// MAXQ*32 >= d.  Returns RED_SUCCESS or the failing status (warp-uniform).
-template <int MAXQ, bool COOP = false>
-__device__ inline int warp_babai(const View &v, WarpSmem &s, int kappa, int sr_end, int sr_start, double eta, int lane,
+// MAXQ*32 >= d.  Returns RED_SUCCESS or the failing status (warp-uniform).  XF: the handle tracks U, whose row kappa
+// takes the same integer row operations as b's.
+template <int MAXQ, bool COOP, bool XF>
+__device__ inline int warp_babai(const LLLView<XF> &v, WarpSmem &s, int kappa, int sr_end, int sr_start, double eta, int lane,
                                  long &iters, LLLStats *pst = nullptr, CoopShared *C = nullptr)
 {
   long max_expo = LONG_MAX;
@@ -192,22 +193,27 @@ __device__ inline int warp_babai(const View &v, WarpSmem &s, int kappa, int sr_e
     if (COOP && nnz)
     {
       coop_post(C, COOP_IGEMV, kappa, nnz, 0, lane);
-      cta_igemv(*C, kappa, nnz, 0, lane);
+      cta_igemv<XF>(*C, kappa, nnz, 0, lane);
     }
     else if (nnz)
     {
       // lane l owns columns l, l+32, ... of a group of up to 8*32 columns: 4 source rows x 8 column chunks = 32 loads in
-      // flight per round (the source rows are contiguous, every load is a 256-byte coalesced line)
+      // flight per round (the source rows are contiguous, every load is a 256-byte coalesced line).  XF: b's nc columns
+      // are followed by U's d columns (column c >= nc is U's column c - nc: U rows are updated over all d columns).
       const int nc           = v.meta[M_NKC];
+      const int ncx          = XF ? nc + v.d : nc;
       unsigned long long *bk = (unsigned long long *)(v.b + (size_t)kappa * v.ldb);
-      for (int cg0 = 0; cg0 < nc; cg0 += 256)
+      unsigned long long *uk = nullptr;
+      if constexpr (XF)
+        uk = (unsigned long long *)u_row(v, kappa);
+      for (int cg0 = 0; cg0 < ncx; cg0 += 256)
       {
         unsigned long long acc[8];
 #pragma unroll
         for (int w = 0; w < 8; w++)
         {
           const int c = cg0 + 32 * w + lane;
-          acc[w]      = (c < nc) ? bk[c] : 0ull;
+          acc[w]      = (c < nc) ? bk[c] : (XF && c < ncx) ? uk[c - nc] : 0ull;
         }
         for (int t0 = 0; t0 < nnz; t0 += 4)
         {
@@ -218,19 +224,21 @@ __device__ inline int warp_babai(const View &v, WarpSmem &s, int kappa, int sr_e
           {
             const int t = t0 + u;
             lxv[u] = 0ull, ev[u] = 0;
-            const unsigned long long *src = bk;
+            const unsigned long long *src = bk, *usrc = uk;
             if (t < nnz)
             {
               lxv[u]             = (unsigned long long)__double_as_longlong(s.aux[t]);
               const long long pk = __double_as_longlong(s.murow[t]);
               ev[u]              = (int)(pk >> 32);
               src = (const unsigned long long *)(v.b + (size_t)(int)(pk & 0xffffffffll) * v.ldb);
+              if constexpr (XF)
+                usrc = (const unsigned long long *)u_row(v, (int)(pk & 0xffffffffll));
             }
 #pragma unroll
             for (int w = 0; w < 8; w++)
             {
               const int c = cg0 + 32 * w + lane;
-              bv[u][w]    = (t < nnz && c < nc) ? src[c] : 0ull;
+              bv[u][w]    = (t < nnz && c < nc) ? src[c] : (XF && t < nnz && c < ncx) ? usrc[c - nc] : 0ull;
             }
           }
 #pragma unroll
@@ -248,6 +256,8 @@ __device__ inline int warp_babai(const View &v, WarpSmem &s, int kappa, int sr_e
           const int c = cg0 + 32 * w + lane;
           if (c < nc)
             bk[c] = acc[w];
+          else if (XF && c < ncx)
+            uk[c - nc] = acc[w];
         }
       }
     }
@@ -261,7 +271,7 @@ __device__ inline int warp_babai(const View &v, WarpSmem &s, int kappa, int sr_e
 }
 
 // Matrix::get_max_exp over b with Z_NR<long>::exponent (nr_Z_l.inl:40-48)
-__device__ inline long warp_max_exp_of_b(const View &v, int lane)
+__device__ inline long warp_max_exp_of_b(const ViewCore &v, int lane)
 {
   long mx = 0;
   for (int i = 0; i < v.d; i++)
@@ -284,7 +294,7 @@ __device__ inline long warp_max_exp_of_b(const View &v, int lane)
   return mx;
 }
 
-__device__ inline bool warp_b_row_is_zero(const View &v, int i, int lane)
+__device__ inline bool warp_b_row_is_zero(const ViewCore &v, int i, int lane)
 {
   int nz = 0;
   for (int c = lane; c < v.n; c += 32)
@@ -293,7 +303,7 @@ __device__ inline bool warp_b_row_is_zero(const View &v, int i, int lane)
 }
 
 // get_gram(kappa,kappa) (gso.h:314-331) for the Lovasz test; computes the dot product if the entry is invalid.
-__device__ inline double warp_get_gram_diag(const View &v, WarpSmem &s, int i, int lane)
+__device__ inline double warp_get_gram_diag(const ViewCore &v, WarpSmem &s, int i, int lane)
 {
   double *g  = v.gf + tri_off(i) + i;
   double val = *g;
@@ -318,8 +328,8 @@ __device__ inline double warp_get_gram_diag(const View &v, WarpSmem &s, int i, i
 }
 
 // LLLReduction::size_reduction(kappa_min, kappa_end, size_reduction_start), lll.h:106-122
-template <int MAXQ, bool COOP = false>
-__device__ inline int warp_size_reduction(const View &v, WarpSmem &s, int kappa_min, int kappa_end, int sr_start,
+template <int MAXQ, bool COOP, bool XF>
+__device__ inline int warp_size_reduction(const LLLView<XF> &v, WarpSmem &s, int kappa_min, int kappa_end, int sr_start,
                                           double eta, int lane, long &iters, CoopShared *C = nullptr)
 {
   // Rows below the clean prefix are size-reduced with a valid GSO and untouched since: on them the reference's loop
@@ -332,7 +342,7 @@ __device__ inline int warp_size_reduction(const View &v, WarpSmem &s, int kappa_
   {
     if (k > 0)
     {
-      const int st = warp_babai<MAXQ, COOP>(v, s, k, k, sr_start, eta, lane, iters, nullptr, C);
+      const int st = warp_babai<MAXQ, COOP, XF>(v, s, k, k, sr_start, eta, lane, iters, nullptr, C);
       if (st != RED_SUCCESS)
         return st;
     }
@@ -358,9 +368,10 @@ __device__ inline int warp_size_reduction(const View &v, WarpSmem &s, int kappa_
 }
 
 // LLLReduction::lll(kappa_min, kappa_start, kappa_end, size_reduction_start), lll.cpp:44-164; LLL_DEFAULT flags
-// (no siegel, no early reduction, not verbose).  lov = shared array of d+1 doubles.
-template <int MAXQ, bool COOP = false>
-__device__ inline int warp_lll(const View &v, WarpSmem &s, double *lov, double delta, double eta, int kappa_min,
+// (no siegel, no early reduction, not verbose).  lov = shared array of d+1 doubles.  XF: U follows every row operation
+// (only integer rows change; no decision reads U).
+template <int MAXQ, bool COOP, bool XF>
+__device__ inline int warp_lll(const LLLView<XF> &v, WarpSmem &s, double *lov, double delta, double eta, int kappa_min,
                                int kappa_start, int kappa_end, int sr_start, int lane, LLLStats &st,
                                CoopShared *C = nullptr)
 {
@@ -381,7 +392,7 @@ __device__ inline int warp_lll(const View &v, WarpSmem &s, double *lov, double d
   __syncwarp();
   for (; zeros < d && warp_b_row_is_zero(v, 0, lane); zeros++)
   {
-    lll_move_row<COOP>(v, kappa_min, kappa_end - 1 - zeros, lane, C);
+    lll_move_row<COOP, XF>(v, kappa_min, kappa_end - 1 - zeros, lane, C);
     lll_mu_reload<COOP>(C, kappa_min, kappa_end - 1 - zeros, lane);
   }
   if (zeros < d)
@@ -389,7 +400,7 @@ __device__ inline int warp_lll(const View &v, WarpSmem &s, double *lov, double d
     if (kappa_start > 0)
     {
       const int bst =
-          warp_babai<MAXQ, COOP>(v, s, kappa_start, kappa_start, sr_start, eta, lane, st.babai_iters, nullptr, C);
+          warp_babai<MAXQ, COOP, XF>(v, s, kappa_start, kappa_start, sr_start, eta, lane, st.babai_iters, nullptr, C);
       if (bst != RED_SUCCESS)
       {
         st.final_kappa = kappa_start, st.zeros = zeros;
@@ -425,7 +436,7 @@ __device__ inline int warp_lll(const View &v, WarpSmem &s, double *lov, double d
     const long long cu_ = st.cyc_update;
 #endif
     const int bst =
-        warp_babai<MAXQ, COOP>(v, s, kappa, kappa, sr_start, eta, lane, st.babai_iters, &st, C);
+        warp_babai<MAXQ, COOP, XF>(v, s, kappa, kappa, sr_start, eta, lane, st.babai_iters, &st, C);
 #ifdef B200_LLL_PROFILE
     st.cyc_babai += (clock64() - tb_) - (st.cyc_update - cu_);
     const long long tl_ = clock64();
@@ -476,14 +487,14 @@ __device__ inline int warp_lll(const View &v, WarpSmem &s, double *lov, double d
       const int old_k = kappa;
       if (action == 1)
       {
-        lll_move_row<COOP>(v, old_k, new_kappa, lane, C);
+        lll_move_row<COOP, XF>(v, old_k, new_kappa, lane, C);
         lll_mu_reload<COOP>(C, new_kappa, old_k, lane);
         kappa = new_kappa;
       }
       else
       {
         zeros++;
-        lll_move_row<COOP>(v, old_k, kappa_end - zeros, lane, C);
+        lll_move_row<COOP, XF>(v, old_k, kappa_end - zeros, lane, C);
         lll_mu_reload<COOP>(C, old_k, kappa_end - zeros, lane);
         kappa = old_k;
         continue;

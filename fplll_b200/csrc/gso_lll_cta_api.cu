@@ -3,7 +3,8 @@
 
 namespace {
 
-template <int MAXQ>
+// XF: the handle tracks the transform U (B200GSO_TRANSFORM); the untransformed instantiations never touch it
+template <int MAXQ, bool XF>
 __global__ void __launch_bounds__(CTA_WARPS * 32)
     k_lll_cta(Batch S, int mode, double delta, double eta, int kmin, int kstart, int kend, int sr_start, int *status,
               long *stats, int mu_panels)
@@ -17,10 +18,10 @@ __global__ void __launch_bounds__(CTA_WARPS * 32)
   double *bm        = smem + per + ((sizeof(CoopShared) + 15) / 16) * 2;
   if (w != 0)
   {
-    coop_helper_loop(*C, w, lane);
+    coop_helper_loop<XF>(*C, w, lane);
     return;
   }
-  View v = S.view(l);
+  LLLView<XF> v = S.view(l);
   WarpSmem s;
   s.carve(smem, S.d, S.n, true);
   double *lov = smem + base;
@@ -29,6 +30,8 @@ __global__ void __launch_bounds__(CTA_WARPS * 32)
   if (lane == 0)
   {
     C->v = v;
+    if constexpr (XF)
+      C->u = v.u;
     C->s = s;
     C->bm = bm;
     C->pub = bm + (size_t)((S.d + 32 + 1) & ~1);
@@ -52,9 +55,9 @@ __global__ void __launch_bounds__(CTA_WARPS * 32)
   st.n_swaps = st.final_kappa = st.zeros = st.babai_iters = 0;
   int r;
   if (mode == 0)
-    r = warp_lll<MAXQ, true>(v, s, lov, delta, eta, kmin, kstart, kend, sr_start, lane, st, C);
+    r = warp_lll<MAXQ, true, XF>(v, s, lov, delta, eta, kmin, kstart, kend, sr_start, lane, st, C);
   else
-    r = warp_size_reduction<MAXQ, true>(v, s, kmin, kend, sr_start, eta, lane, st.babai_iters, C);
+    r = warp_size_reduction<MAXQ, true, XF>(v, s, kmin, kend, sr_start, eta, lane, st.babai_iters, C);
   coop_post(C, COOP_EXIT, 0, 0, 0, lane);
   mc.store(v, lane);
   if (lane == 0)
@@ -92,9 +95,11 @@ int b200gso_lll_cta_attrs(int d, int n)
 {
   (void)d, (void)n;  // process-wide kernels: always the opt-in maximum (a smaller handle must not lower it)
   const int sm = SMEM_OPTIN_MAX;
-  CK(cudaFuncSetAttribute((const void *)k_lll_cta<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm));
-  CK(cudaFuncSetAttribute((const void *)k_lll_cta<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm));
-  CK(cudaFuncSetAttribute((const void *)k_lll_cta<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm));
+  const void *fns[] = {(const void *)k_lll_cta<4, false>, (const void *)k_lll_cta<8, false>,
+                       (const void *)k_lll_cta<16, false>, (const void *)k_lll_cta<4, true>,
+                       (const void *)k_lll_cta<8, true>,  (const void *)k_lll_cta<16, true>};
+  for (const void *f : fns)
+    CK(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, sm));
   return 0;
 }
 
@@ -118,11 +123,21 @@ int b200gso_lll_cta_launch(b200gso *h, int mode, double delta, double eta, int k
     mu_panels++;
   }
   sm += used * sizeof(double);
+#define CTA_LAUNCH(Q, XF) \
+  k_lll_cta<Q, XF><<<S.B, CTA_WARPS * 32, sm, h->stream>>>(S, mode, delta, eta, kmin, kstart, kend, sr_start, d_st, d_stats, mu_panels)
+  const bool xf = S.u != nullptr;
   if (S.d <= 128)
-    k_lll_cta<4><<<S.B, CTA_WARPS * 32, sm, h->stream>>>(S, mode, delta, eta, kmin, kstart, kend, sr_start, d_st, d_stats, mu_panels);
+  {
+    if (xf) CTA_LAUNCH(4, true); else CTA_LAUNCH(4, false);
+  }
   else if (S.d <= 256)
-    k_lll_cta<8><<<S.B, CTA_WARPS * 32, sm, h->stream>>>(S, mode, delta, eta, kmin, kstart, kend, sr_start, d_st, d_stats, mu_panels);
+  {
+    if (xf) CTA_LAUNCH(8, true); else CTA_LAUNCH(8, false);
+  }
   else
-    k_lll_cta<16><<<S.B, CTA_WARPS * 32, sm, h->stream>>>(S, mode, delta, eta, kmin, kstart, kend, sr_start, d_st, d_stats, mu_panels);
+  {
+    if (xf) CTA_LAUNCH(16, true); else CTA_LAUNCH(16, false);
+  }
+#undef CTA_LAUNCH
   return 0;
 }

@@ -33,7 +33,7 @@ struct WarpSmem
 };
 
 // Row `idx` (and possibly everything after it) has been modified: the "already reduced" prefix ends there.
-__device__ inline void lower_clean(const View &v, int idx, int lane)
+__device__ inline void lower_clean(const ViewCore &v, int idx, int lane)
 {
   if (lane == 0)
   {
@@ -156,7 +156,7 @@ template <bool SUB, bool PREFIX> __device__ inline double serial_chain(double a,
 }
 
 // MatGSO::update_bf(i), gso.cpp:24-48 for Z_NR<long> (get_f_exp = frexp((double)x), nr_Z_misc.inl:17-22)
-__device__ inline void warp_update_bf(const View &v, int i, int lane)
+__device__ inline void warp_update_bf(const ViewCore &v, int i, int lane)
 {
   const int n = max(v.meta[M_NKC], v.irs[i]);
   const int64_t *brow = v.b + (size_t)i * v.ldb;
@@ -187,7 +187,7 @@ __device__ inline void warp_update_bf(const View &v, int i, int lane)
 }
 
 // invalidate_gram_row, gso.cpp:50-54
-__device__ inline void warp_invalidate_gram_row(const View &v, int i, int lane)
+__device__ inline void warp_invalidate_gram_row(const ViewCore &v, int i, int lane)
 {
   double *g = v.gf + tri_off(i);
   for (int j = lane; j <= i; j += 32)
@@ -195,7 +195,7 @@ __device__ inline void warp_invalidate_gram_row(const View &v, int i, int lane)
 }
 
 // discover_row, gso.cpp:56-82 (float Gram)
-__device__ inline void warp_discover_row(const View &v, int lane)
+__device__ inline void warp_discover_row(const ViewCore &v, int lane)
 {
   const int i = v.meta[M_NKR];
   __syncwarp();
@@ -217,7 +217,7 @@ __device__ inline void warp_discover_row(const View &v, int lane)
 // re-derived from the contiguous int64 row instead: update_bf (gso.cpp:24-48) stores frexp/ldexp of (double)b(i,c),
 // which is exactly (double)b(i,c) * 2^-row_expo[i] (power-of-two scaling is exact), hence bit-identical.
 // Precondition (the reference's !in_row_op_range(i) assert, gso.h:316): row_op_end has run since b[i] last changed.
-__device__ inline void stage_bf_row(const View &v, int i, int ncols, double *vb, int first, int step)
+__device__ inline void stage_bf_row(const ViewCore &v, int i, int ncols, double *vb, int first, int step)
 {
   if (v.host_basis)
   {
@@ -232,7 +232,7 @@ __device__ inline void stage_bf_row(const View &v, int i, int ncols, double *vb,
   for (int c = first; c < ncols; c += step)
     vb[c] = __dmul_rn((double)brow[c], sc);
 }
-__device__ inline void warp_stage_bf_row(const View &v, int i, int ncols, double *vb, int lane)
+__device__ inline void warp_stage_bf_row(const ViewCore &v, int i, int ncols, double *vb, int lane)
 {
   stage_bf_row(v, i, ncols, vb, lane, 32);
 }
@@ -305,7 +305,7 @@ __device__ inline double lane_dot(const double *__restrict__ bfcol /* &bf(j,0) *
 // r(i,k) for k outside the panel comes from shared memory (rrow), inside the panel by shuffle from the lane that
 // has just finished its own chain — the "right-looking" schedule that keeps every chain in reference order.
 // Returns false (warp-uniform) if some mu(i,j) is not finite; gso_valid_cols[i] is then left unchanged.
-__device__ inline bool warp_update_gso_row(const View &v, int i, int last_j, WarpSmem &s, int lane)
+__device__ inline bool warp_update_gso_row(const ViewCore &v, int i, int last_j, WarpSmem &s, int lane)
 {
   if (i >= v.meta[M_NKR])
     warp_discover_row(v, lane);
@@ -432,7 +432,7 @@ __device__ inline bool warp_update_gso_row(const View &v, int i, int last_j, War
 }
 
 // row_op_end(first,last), gso_interface.cpp:32-53
-__device__ inline void warp_row_op_end(const View &v, int first, int last, int lane)
+__device__ inline void warp_row_op_end(const ViewCore &v, int first, int last, int lane)
 {
   const int nkr = v.meta[M_NKR];
   for (int i = first; i < last; i++)
@@ -451,8 +451,12 @@ __device__ inline void warp_row_op_end(const View &v, int first, int last, int l
   __syncwarp();
 }
 
+// Row i of the transform U (B200GSO_TRANSFORM handles): d columns, row stride ld_b(d).
+__device__ inline int64_t *u_row(const View &v, int i) { return v.u + (size_t)i * ld_b(v.d); }
+
 // row_addmul_we(i, j, x, expo_add), gso.cpp:236-262 -> row_add/row_sub/row_addmul_si/row_addmul_si_2exp
-// (gso.cpp:84-195, numvect.h:268-341) on b only (u, u_inv_t empty in the BKZ regime).  int64 wraps like Z_NR<long>.
+// (gso.cpp:84-195, numvect.h:268-341) on b over n_known_cols, and on U (when the handle has one) over all d columns:
+// the reference's u[i].addmul_si(u[j], x) has no length bound.  u_inv_t is not kept.  int64 wraps like Z_NR<long>.
 __device__ inline void warp_row_addmul_we(const View &v, int i, int j, double x, long expo_add, int lane)
 {
   long expo;
@@ -473,10 +477,20 @@ __device__ inline void warp_row_addmul_we(const View &v, int i, int j, double x,
       unsigned long long t = bj[c] * ux;
       bi[c] += (expo >= 64 ? 0ull : (t << expo));
     }
+  if (v.u)
+  {
+    unsigned long long *ui       = (unsigned long long *)u_row(v, i);
+    const unsigned long long *uj = (const unsigned long long *)u_row(v, j);
+    for (int c = lane; c < v.d; c += 32)
+    {
+      unsigned long long t = uj[c] * ux;
+      ui[c] += (expo >= 64 ? 0ull : (t << expo));
+    }
+  }
   __syncwarp();
 }
 
-// row_swap(i,j), gso.cpp:264-287: integer rows only
+// row_swap(i,j), gso.cpp:264-287: integer rows only (b, and U when the handle has one)
 __device__ inline void warp_row_swap(const View &v, int i, int j, int lane)
 {
   int64_t *a = v.b + (size_t)i * v.ldb, *b = v.b + (size_t)j * v.ldb;
@@ -486,6 +500,16 @@ __device__ inline void warp_row_swap(const View &v, int i, int j, int lane)
     int64_t t = a[c];
     a[c]      = b[c];
     b[c]      = t;
+  }
+  if (v.u)
+  {
+    int64_t *ua = u_row(v, i), *ub = u_row(v, j);
+    for (int c = lane; c < v.d; c += 32)
+    {
+      int64_t t = ua[c];
+      ua[c]     = ub[c];
+      ub[c]     = t;
+    }
   }
   __syncwarp();
 }
@@ -547,11 +571,11 @@ template <class T, class At> __device__ inline void rotate_seq(At at, int lo, in
   }
 }
 
-// move_row(old_r, new_r), gso.cpp:289-366 (float Gram, no transforms).  Rotations of mu, r, b, bf, row_expo,
+// move_row(old_r, new_r), gso.cpp:289-366 (float Gram; U: warp_move_u_row).  Rotations of mu, r, b, bf, row_expo,
 // gso_valid_cols are done column-by-column (each lane carries one column through the rotated rows, no scratch);
 // only the entries that can still be valid after the call (columns < min(old,new), SURVEY Appendix A) are moved
 // for mu and r.  The symmetric row+column rotation of gf (matrix.cpp:65-93) goes through v.scratch.
-__device__ inline void warp_move_row(const View &v, int old_r, int new_r, int lane)
+__device__ inline void warp_move_row(const ViewCore &v, int old_r, int new_r, int lane)
 {
   if (old_r == new_r)
     return;
@@ -625,8 +649,31 @@ __device__ inline void warp_move_row(const View &v, int old_r, int new_r, int la
   __syncwarp();
 }
 
+// The U half of move_row(old_r, new_r) (gso.cpp:289-366: u.rotate_right / u.rotate_left): rows [lo..hi] of U rotate
+// like those of b.  Kept apart from warp_move_row, which the untransformed LLL kernels share.
+__device__ inline void warp_move_u_row(const View &v, int old_r, int new_r, int lane)
+{
+  const bool right = new_r < old_r;
+  const int lo = right ? new_r : old_r, hi = right ? old_r : new_r;
+  for (int c = lane; c < v.d; c += 32)
+    rotate_seq<int64_t>([&](int i) -> int64_t & { return u_row(v, i)[c]; }, lo, hi, right);
+  __syncwarp();
+}
+
+// negate_row_of_b(i), gso.h:291-311, on b and, unlike the reference (which leaves u alone), on U too: a handle's U
+// always satisfies U * B_in = B.
+__device__ inline void warp_negate_row(const View &v, int i, int lane)
+{
+  lower_clean(v, i, lane);
+  for (int c = lane; c < v.n; c += 32)
+    v.b[(size_t)i * v.ldb + c] = -v.b[(size_t)i * v.ldb + c];
+  if (v.u)
+    for (int c = lane; c < v.d; c += 32)
+      u_row(v, i)[c] = -u_row(v, i)[c];
+}
+
 // set_r(i,j,f), gso_interface.h:739-746
-__device__ inline void warp_set_r(const View &v, int i, int j, double f, int lane)
+__device__ inline void warp_set_r(const ViewCore &v, int i, int j, double f, int lane)
 {
   if (lane == 0)
   {

@@ -8,6 +8,7 @@ import numpy as np
 from ._lib import B200Error, load
 
 GSO_DEFAULT, GSO_INT_GRAM, GSO_ROW_EXPO, GSO_OP_FORCE_LONG = 0, 1, 2, 4  # gso_interface.h:26-32
+GSO_TRANSFORM = 512  # include/b200gso.h B200GSO_TRANSFORM (not a reference value): the handle keeps U
 RED_SUCCESS, RED_GSO_FAILURE, RED_BABAI_FAILURE, RED_LLL_FAILURE = 0, 2, 3, 4  # defs.h:153-169
 # b200gso_op types (include/b200gso.h)
 OP_ROW_ADDMUL, OP_MOVE_ROW, OP_ROW_SWAP, OP_ROW_OP_END, OP_NEGATE = 1, 2, 3, 4, 5
@@ -32,6 +33,8 @@ def _lib():
         L.b200gso_set_basis_dev.argtypes = [vp, vp]
         L.b200gso_get_basis.argtypes = [vp, i64p]
         L.b200gso_upload_row.argtypes = [vp, i, i64p]
+        L.b200gso_set_transform.argtypes = [vp, i64p]
+        L.b200gso_get_transform.argtypes = [vp, i64p]
         L.b200gso_discover_all_rows.argtypes = [vp]
         L.b200gso_update_gso_row.argtypes = [vp, i, i, ip]
         L.b200gso_update_gso.argtypes = [vp, ip]
@@ -68,19 +71,28 @@ def _ptr(a, ct):
 
 
 class MatGSO:
-    """MatGSO(b, flags): b is (d, n) or (batch, d, n) int64.  u / u_inv_t are not supported (empty in the BKZ
-    regime, bkz.cpp:826-836); GSO_INT_GRAM raises like an unsupported template instantiation."""
+    """MatGSO(b, flags, device, u): b is (d, n) or (batch, d, n) int64.  u (d, d) or (batch, d, d) int64 makes it a
+    transform object like the reference's MatGSO(b, u, u_inv_t = {}, flags) with a non-empty u (enable_transform): U
+    starts as u and takes every integer row operation applied to b (.u reads it back).  GSO_TRANSFORM in flags without
+    u starts U at the identity.  One intended divergence from the reference: negate_row_of_b / OP_NEGATE negate the row
+    of U too, so that U * B_in == B always holds (include/b200gso.h).  u_inv_t is not supported; GSO_INT_GRAM raises
+    like an unsupported template instantiation."""
 
-    def __init__(self, b, flags=GSO_ROW_EXPO, device=0):
+    def __init__(self, b, flags=GSO_ROW_EXPO, device=0, u=None):
         b = np.ascontiguousarray(b, dtype=np.int64)
         if b.ndim == 2:
             b = b[None]
         self.batch, self.d, self.n = b.shape
+        if u is not None:
+            flags |= GSO_TRANSFORM
         self.flags = flags
         self.enable_row_expo = bool(flags & GSO_ROW_EXPO)
+        self.enable_transform = bool(flags & GSO_TRANSFORM)
         self._h = C.c_void_p()
         _ck(_lib().b200gso_create(C.byref(self._h), self.batch, self.d, self.n, flags, device), "b200gso_create")
         _ck(_lib().b200gso_set_basis(self._h, _ptr(b, C.c_int64)), "b200gso_set_basis")
+        if u is not None:
+            self.set_transform(u)
 
     def close(self):
         if getattr(self, "_h", None) and self._h.value:
@@ -166,7 +178,19 @@ class MatGSO:
         rows = np.ascontiguousarray(rows, dtype=np.int64).reshape(self.batch, self.n)
         _ck(_lib().b200gso_upload_row(self._h, i, _ptr(rows, C.c_int64)), "upload_row")
 
+    def set_transform(self, u):
+        """replaces U: (d, d) (every lattice) or (batch, d, d) int64"""
+        u = np.ascontiguousarray(np.broadcast_to(np.asarray(u, np.int64), (self.batch, self.d, self.d)))
+        _ck(_lib().b200gso_set_transform(self._h, _ptr(u, C.c_int64)), "set_transform")
+
     # ---- state ---------------------------------------------------------------------------------------
+    @property
+    def u(self):
+        """U of a transform object, (batch, d, d) int64"""
+        out = np.empty((self.batch, self.d, self.d), np.int64)
+        _ck(_lib().b200gso_get_transform(self._h, _ptr(out, C.c_int64)), "get_transform")
+        return out
+
     @property
     def b(self):
         out = np.empty((self.batch, self.d, self.n), np.int64)
@@ -247,20 +271,32 @@ class MatGSO:
         _ck(_lib().b200gso_sync(self._h), "sync")
 
 
-def lll_reduction(b, delta=0.99, eta=0.51, device=0):
-    """lll_reduction(ZZ_mat<long>& b, delta, eta, LM_FAST, FT_DOUBLE) (wrapper.h:136-157, wrapper.cpp:538-553):
-    reduces b IN PLACE (numpy int64 array (d,n) or (batch,d,n)); returns RedStatus (int or array)."""
+def lll_reduction(b, delta=0.99, eta=0.51, device=0, u=None):
+    """lll_reduction(ZZ_mat<long>& b, [u,] delta, eta, LM_FAST, FT_DOUBLE) (wrapper.h:136-157, wrapper.cpp:538-553):
+    reduces b IN PLACE (numpy int64 array (d,n) or (batch,d,n)); returns RedStatus (int or array).  u ((d,d) or
+    (batch,d,d) int64) is overwritten with the transform of the whole call, U * b_in == b_out (the reference starts it
+    at the identity, u.gen_identity(d) in FPLLL_DEFINE_LLL)."""
     arr = np.asarray(b)
-    m = MatGSO(arr, GSO_ROW_EXPO | GSO_OP_FORCE_LONG, device)
+    d = arr.shape[-2]
+    m = MatGSO(arr, GSO_ROW_EXPO | GSO_OP_FORCE_LONG, device, u=None if u is None else np.eye(d, dtype=np.int64))
     st, _ = m.lll(delta, eta)
     out = m.b
+    uo = m.u if u is not None else None
     m.close()
-    # zeros_first (wrapper.cpp:732, util.cpp:257-287): zero rows parked at the end by LLL move to the front
+    # zeros_first (wrapper.cpp:732, util.cpp:257-287): zero rows parked at the end by LLL move to the front, and the
+    # rows of u move with them
     for l in range(out.shape[0]):
         nz = np.any(out[l] != 0, axis=1)
-        out[l] = np.concatenate([out[l][~nz], out[l][nz]], axis=0)
+        perm = np.concatenate([np.flatnonzero(~nz), np.flatnonzero(nz)])
+        out[l] = out[l][perm]
+        if uo is not None:
+            uo[l] = uo[l][perm]
     if arr.ndim == 2:
         b[...] = out[0]
+        if u is not None:
+            u[...] = uo[0]
         return int(st[0])
     b[...] = out
+    if u is not None:
+        u[...] = uo
     return st

@@ -88,6 +88,13 @@ int b200bkz_add_strategy(b200bkz_t *h, int block_size, const int *preproc, int n
                          const double *expectation, const double *coefficients, int n_prune);
 /* bkz_reduction on a d x n int64 basis, in place.  Returns 0 or a negative error; RedStatus in stats->status. */
 int b200bkz_reduce(b200bkz_t *h, int d, int n, int64_t *b, const b200bkz_param *param, b200bkz_stats *stats);
+/* bkz_reduction(b, u, param) (bkz.h:357-426, BKZReduction with a transform, bkz.cpp:822-836): the same call, and u
+ * (d x d int64, row-major, in/out) takes every integer row operation applied to b.  The caller initialises u as for
+ * BKZReduction (bkz_reduction itself starts it at the identity, bkz.cpp:857-859).  Same b, status and statistics as
+ * b200bkz_reduce; u differs from the reference's where the reference negates a row of b without u (B200GSO_TRANSFORM in
+ * b200gso.h), so that U * B_in = B_out always holds here. */
+int b200bkz_reduce_transform(b200bkz_t *h, int d, int n, int64_t *b, int64_t *u, const b200bkz_param *param,
+                             b200bkz_stats *stats);
 const char *b200bkz_last_error(void);
 /* get_slide_potential(start_row, end_row, block_size) (gso_interface.cpp:244-258) of an r diagonal given as mantissa /
  * exponent pairs (rows 0 .. end_row - 1): what slide reduction's termination test compares tour to tour. */

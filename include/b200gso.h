@@ -36,6 +36,17 @@ typedef struct b200gso b200gso_t;
  * operation itself and ships the refreshed floating-point row with b200gso_upload_row_fp; the int64 entry points
  * (set_basis, row_addmul_we, upload_row, device LLL) are rejected on such a handle. */
 #define B200GSO_HOST_BASIS 256
+/* Not a reference value.  The handle also keeps the transform U of MatGSO(b, u, u_inv_t = {}, flags) (gso.h:113-130,
+ * enable_transform): int64, d x d per lattice, starting as the identity.  Every integer row operation on b — row_addmul_we
+ * with its 2^expo shift, row_swap, move_row, and the device LLL / size reduction / op lists — is applied to the row of U
+ * with the same index, with the same wrapping int64 arithmetic as Z_NR<long>, over all d columns of U (the reference's
+ * u[i].addmul_si(u[j], x) has no n_known_cols bound).  No decision reads U: a transform handle ends every call with the
+ * same b, GSO state, status and statistics as a handle without it.
+ * One intended divergence: negate_row_of_b (b200gso_negate_row_of_b, B200GSO_OP_NEGATE) negates row i of U together with
+ * row i of b.  The reference's negate_row_of_b (gso.h:291-311) negates b only, so after it the reference's U no longer
+ * satisfies U * B_in = B; here that identity always holds.
+ * Not with B200GSO_HOST_BASIS (B200GSO_EINVAL).  U^-T (u_inv_t) is not kept. */
+#define B200GSO_TRANSFORM 512
 
 /* RedStatus, fplll/defs.h:153-169 */
 #define B200_RED_SUCCESS 0
@@ -64,8 +75,14 @@ int b200gso_set_basis_dev(b200gso_t *h, const int64_t *dev_b);
 int b200gso_get_basis(b200gso_t *h, int64_t *b);
 
 /* Uploads replacement contents for row i of every lattice (batch*n int64) — the protocol of SURVEY §7 for a host
- * that performs the integer row operation itself: equivalent to writing b[i] then row_op_end(i, i+1). */
+ * that performs the integer row operation itself: equivalent to writing b[i] then row_op_end(i, i+1).
+ * B200GSO_EINVAL on a B200GSO_TRANSFORM handle: the device cannot know how the host's operation changed U. */
 int b200gso_upload_row(b200gso_t *h, int i, const int64_t *rows);
+
+/* B200GSO_TRANSFORM handles only (B200GSO_EINVAL otherwise): replace U / read U back, batch*d*d int64, row-major,
+ * lattice-major.  set_basis leaves U alone. */
+int b200gso_set_transform(b200gso_t *h, const int64_t *u);
+int b200gso_get_transform(b200gso_t *h, int64_t *u);
 
 /* MatGSOInterface::discover_all_rows, gso_interface.h:761-765 */
 int b200gso_discover_all_rows(b200gso_t *h);
@@ -127,7 +144,8 @@ int b200gso_lll_range(b200gso_t *h, double delta, double eta, int kappa_min, int
 /* LLLReduction::size_reduction(kappa_min, kappa_end, size_reduction_start), lll.h:106-122.  status[l] = RedStatus. */
 int b200gso_size_reduction(b200gso_t *h, double eta, int kappa_min, int kappa_end, int size_reduction_start,
                            int *status);
-/* MatGSO::negate_row_of_b(i), gso.h:291-297 (bracket with row_op_begin/end like the reference's callers). */
+/* MatGSO::negate_row_of_b(i), gso.h:291-297 (bracket with row_op_begin/end like the reference's callers).  On a
+ * B200GSO_TRANSFORM handle row i of U is negated too (see B200GSO_TRANSFORM: the reference leaves u alone). */
 int b200gso_negate_row_of_b(b200gso_t *h, int i);
 /* What Enumeration pulls out of the GSO for block [first, first+beta) of lattice `lattice` (enumerate.cpp:91-141,
  * enumerate_ext.cpp:91-148): mut[k*beta+j] = get_mu(first+j, first+k) for j > k (true value, row exponents applied)
