@@ -17,6 +17,7 @@
 #include <algorithm>
 #include <math_constants.h>
 #include <string>
+#include <utility>
 #include <vector>
 
 namespace {
@@ -46,6 +47,9 @@ struct HBatch
   long *ensb;
 };
 
+// which matrices a kernel instantiation updates next to b (a template parameter, chosen at launch from the handle)
+enum { HT_NONE = 0, HT_U = 1, HT_UINV = 2 };
+
 struct HView
 {
   int d, n, ldb, row_expo_en, keep_hist;
@@ -54,6 +58,30 @@ struct HView
   int *row_expo, *irs, *meta, *hslot;
   long *ensb;
 };
+
+// B200HH_TRANSFORM / B200HH_INV_TRANSFORM: U and U^-T, dense d x d per lattice (nullptr unless the flags ask).  They are
+// the LAST kernel argument of hk_size_reduce, hk_swap and hk_hlll rather than fields of HBatch: a bigger HBatch moves
+// the arguments behind it and changes how the compiler reads the struct (past 128 bytes it is no longer taken apart into
+// registers), so the instantiations without a transform would no longer compile to the code they had before U existed.
+// It travels down by value (a reference to it also changed their code).
+struct HTr
+{
+  int64_t *u, *uinvt;
+};
+
+// U and U^-T of the calling warp's lattice (both nullptr when TR == HT_NONE)
+template <int TR> __device__ inline HTr htr(const HBatch &S, HTr T)
+{
+  HTr t{nullptr, nullptr};
+  if (TR != HT_NONE)
+  {
+    const size_t l = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), dd = (size_t)S.d * S.d;
+    t.u = T.u + l * dd;
+    if (TR == HT_UINV)
+      t.uinvt = T.uinvt + l * dd;
+  }
+  return t;
+}
 
 __device__ inline HView hview(const HBatch &S, int l)
 {
@@ -315,8 +343,26 @@ __device__ inline void w_update_R(const HView &v, int i, int last_j, double *sR,
 
 __device__ inline long hfexpo(double x) { return (long)ilogb(x) + 1; }
 
-// size_reduce(k, end, start), householder.cpp:403-451 with row_addmul_we, :522-559
-__device__ inline bool w_size_reduce(const HView &v, int k, int sr_end, int sr_start, int lane)
+// row a += (x * 2^expo) * row c of a dense d x d int64 matrix, all d columns, wrapping: Z_NR<long>'s addmul_si and
+// addmul_si_2exp as row_add / row_sub / row_addmul_si / row_addmul_si_2exp apply them to u and u_inv_t
+// (householder.cpp:455-520: no n_known_cols bound there)
+__device__ inline void w_mat_addmul(int64_t *m, int d, int a, int c, unsigned long long x, long expo, int lane)
+{
+  unsigned long long *ra = (unsigned long long *)(m + (size_t)a * d);
+  const unsigned long long *rc = (const unsigned long long *)(m + (size_t)c * d);
+  for (int col = lane; col < d; col += 32)
+  {
+    unsigned long long t = rc[col] * x;
+    if (expo)
+      t = expo >= 64 ? 0ull : (t << expo);
+    ra[col] += t;
+  }
+}
+
+// size_reduce(k, end, start), householder.cpp:403-451 with row_addmul_we, :522-559.  TR >= HT_U: U[k] += lx 2^expo U[i];
+// TR == HT_UINV also U^-T[i] -= lx 2^expo U^-T[k], with the lx and expo of b's update.
+template <int TR>
+__device__ inline bool w_size_reduce(const HView &v, HTr t, int k, int sr_end, int sr_start, int lane)
 {
   const int n = v.n, nc = v.meta[HM_NKC];
   double *Rk          = v.R + (size_t)k * n;
@@ -344,6 +390,10 @@ __device__ inline bool w_size_reduce(const HView &v, int k, int sr_end, int sr_s
           t = expo >= 64 ? 0ull : (t << expo);
         bk[c] += t;
       }
+      if (TR >= HT_U)
+        w_mat_addmul(t.u, v.d, k, i, lx, expo, lane);
+      if (TR == HT_UINV)
+        w_mat_addmul(t.uinvt, v.d, i, k, 0ull - lx, expo, lane);
       for (int c = lane; c < i; c += 32)
       {
         if (f == 1.0)
@@ -457,19 +507,31 @@ __global__ void hk_update_R_last(HBatch S, int i)
   if (hsetup(S, v, sR, sP, lane))
     w_update_R_last(v, i, sP, lane);
 }
-__global__ void hk_size_reduce(HBatch S, int k, int e, int st, int *reduced)
+template <int TR> __global__ void hk_size_reduce(HBatch S, int k, int e, int st, int *reduced, HTr T)
 {
   HView v;
   double *sR, *sP;
   int lane;
   if (!hsetup(S, v, sR, sP, lane))
     return;
-  const bool r = w_size_reduce(v, k, e, st, lane);
+  const bool r = w_size_reduce<TR>(v, htr<TR>(S, T), k, e, st, lane);
   if (reduced && lane == 0)
     reduced[blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)] = r ? 1 : 0;
 }
-// swap(i, j), householder.cpp:372-398
-__device__ inline void w_swap(const HView &v, int i, int j, int lane)
+// rows i and j of a dense d x d int64 matrix
+__device__ inline void w_mat_swap(int64_t *m, int d, int i, int j, int lane)
+{
+  for (int c = lane; c < d; c += 32)
+  {
+    const int64_t t    = m[(size_t)i * d + c];
+    m[(size_t)i * d + c] = m[(size_t)j * d + c];
+    m[(size_t)j * d + c] = t;
+  }
+}
+
+// swap(i, j), householder.cpp:372-398, with rows i and j of U (TR >= HT_U) and of U^-T (TR == HT_UINV)
+template <int TR>
+__device__ inline void w_swap(const HView &v, HTr t, int i, int j, int lane)
 {
   if (lane == 0 && i < v.meta[HM_NKR])
     v.meta[HM_NKR] = i;  // invalidate_row(i)
@@ -482,6 +544,10 @@ __device__ inline void w_swap(const HView &v, int i, int j, int lane)
     v.bf[(size_t)i * v.n + c] = v.bf[(size_t)j * v.n + c];
     v.bf[(size_t)j * v.n + c] = f;
   }
+  if (TR >= HT_U)
+    w_mat_swap(t.u, v.d, i, j, lane);
+  if (TR == HT_UINV)
+    w_mat_swap(t.uinvt, v.d, i, j, lane);
   if (lane == 0)
   {
     double t = v.sigma[i];
@@ -502,13 +568,13 @@ __device__ inline void w_swap(const HView &v, int i, int j, int lane)
   }
   __syncwarp();
 }
-__global__ void hk_swap(HBatch S, int i, int j)
+template <int TR> __global__ void hk_swap(HBatch S, int i, int j, HTr T)
 {
   HView v;
   double *sR, *sP;
   int lane;
   if (hsetup(S, v, sR, sP, lane))
-    w_swap(v, i, j, lane);
+    w_swap<TR>(v, htr<TR>(S, T), i, j, lane);
 }
 // recover_R(i), householder.h:597-608
 __device__ inline void w_recover_R(const HView &v, int i, int lane)
@@ -543,7 +609,8 @@ struct HlllArgs
 };
 
 // size_reduction(kappa, kappa, 0), hlll.cpp:262-354 (default branch: approx = 0.1)
-template <int NPL> __device__ inline void w_hlll_size_reduction(const HView &v, int kappa, double *sR, double *sP, int lane)
+template <int NPL, int TR>
+__device__ inline void w_hlll_size_reduction(const HView &v, HTr t, int kappa, double *sR, double *sP, int lane)
 {
   bool prev_not_stop = true;
   w_update_R<NPL>(v, kappa, 0, sR, sP, lane);
@@ -553,7 +620,7 @@ template <int NPL> __device__ inline void w_hlll_size_reduction(const HView &v, 
   __syncwarp();
   for (;;)
   {
-    if (!w_size_reduce(v, kappa, kappa, 0, lane))
+    if (!w_size_reduce<TR>(v, t, kappa, kappa, 0, lane))
       return;
     const double t    = v.nsb[kappa];
     const long expo0  = v.ensb[kappa];
@@ -572,7 +639,8 @@ template <int NPL> __device__ inline void w_hlll_size_reduction(const HView &v, 
   }
 }
 
-template <int NPL> __device__ inline int w_hlll(const HView &v, const HlllArgs &A, int l, double *sR, double *sP, int lane)
+template <int NPL, int TR>
+__device__ inline int w_hlll(const HView &v, HTr t, const HlllArgs &A, int l, double *sR, double *sP, int lane)
 {
   const int d = v.d, n = v.n;
   double *dR = A.dR + (size_t)l * d, *eR = A.eR + (size_t)l * d, *pR = A.prevR + (size_t)l * d;
@@ -603,7 +671,7 @@ template <int NPL> __device__ inline int w_hlll(const HView &v, const HlllArgs &
       status = 9;  // RED_HLLL_FAILURE: iteration guard (the reference has none; protects the device from a livelock)
       break;
     }
-    w_hlll_size_reduction<NPL>(v, k, sR, sP, lane);
+    w_hlll_size_reduction<NPL, TR>(v, t, k, sR, sP, lane);
     // verify_size_reduction(k), hlll.cpp:373-478 (default branch)
     const double *Rk = v.R + (size_t)k * n;
     {
@@ -683,7 +751,7 @@ template <int NPL> __device__ inline int w_hlll(const HView &v, const HlllArgs &
     }
     else
     {
-      w_swap(v, k - 1, k, lane);
+      w_swap<TR>(v, t, k - 1, k, lane);
       prev_k = k;
       if (k - 1 == 0)
       {
@@ -705,7 +773,7 @@ template <int NPL> __device__ inline int w_hlll(const HView &v, const HlllArgs &
   return status;
 }
 
-template <int NPL> __global__ void hk_hlll(HBatch S, HlllArgs A)
+template <int NPL, int TR> __global__ void hk_hlll(HBatch S, HlllArgs A, HTr T)
 {
   HView v;
   double *sR, *sP;
@@ -713,10 +781,18 @@ template <int NPL> __global__ void hk_hlll(HBatch S, HlllArgs A)
   if (!hsetup(S, v, sR, sP, lane))
     return;
   const int l  = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  const int st = w_hlll<NPL>(v, A, l, sR, sP, lane);
+  const int st = w_hlll<NPL, TR>(v, htr<TR>(S, T), A, l, sR, sP, lane);
   if (lane == 0)
     A.status[l] = st;
 }
+// U (and U^-T) = identity on every lattice (the buffers were zeroed)
+__global__ void hk_identity(int64_t *m, int d)
+{
+  int64_t *ml = m + (size_t)blockIdx.x * d * d;
+  for (int i = threadIdx.x; i < d; i += blockDim.x)
+    ml[(size_t)i * d + i] = 1;
+}
+
 __global__ void hk_set_updated(HBatch S, int val)
 {
   const int l = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1068,6 +1144,8 @@ struct b200hh
   unsigned long long *d_hlll_it = nullptr;
   XMaps xmaps;
   int x_state = 0;  // tensor maps of hk_update_R_x32: 0 not built, 1 ready, -1 unavailable
+  int tr = HT_NONE;  // the transform template parameter of hk_size_reduce, hk_swap and hk_hlll
+  HTr T{nullptr, nullptr};  // batch x d x d each
   std::vector<void *> allocs;
 };
 
@@ -1106,6 +1184,54 @@ static bool x_maps(b200hh *h)
   return true;
 }
 
+// the transform instantiations of the kernels that change b
+template <int TR> static cudaError_t hh_kernel_attrs()
+{
+  const void *fns[] = {(const void *)hk_size_reduce<TR>, (const void *)hk_swap<TR>, (const void *)hk_hlll<4, TR>,
+                       (const void *)hk_hlll<8, TR>, (const void *)hk_hlll<14, TR>, (const void *)hk_hlll<32, TR>};
+  for (const void *f : fns)
+  {
+    const cudaError_t e = cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    if (e != cudaSuccess)
+      return e;
+  }
+  return cudaSuccess;
+}
+
+static void launch_size_reduce(const b200hh *h, int k, int e, int st)
+{
+  switch (h->tr)
+  {
+  case HT_NONE: hk_size_reduce<HT_NONE><<<hgrid(h), HW * 32, h->smem, h->stream>>>(h->S, k, e, st, h->d_red, h->T); break;
+  case HT_U: hk_size_reduce<HT_U><<<hgrid(h), HW * 32, h->smem, h->stream>>>(h->S, k, e, st, h->d_red, h->T); break;
+  default: hk_size_reduce<HT_UINV><<<hgrid(h), HW * 32, h->smem, h->stream>>>(h->S, k, e, st, h->d_red, h->T); break;
+  }
+}
+
+static void launch_swap(const b200hh *h, int i, int j)
+{
+  switch (h->tr)
+  {
+  case HT_NONE: hk_swap<HT_NONE><<<hgrid(h), HW * 32, h->smem, h->stream>>>(h->S, i, j, h->T); break;
+  case HT_U: hk_swap<HT_U><<<hgrid(h), HW * 32, h->smem, h->stream>>>(h->S, i, j, h->T); break;
+  default: hk_swap<HT_UINV><<<hgrid(h), HW * 32, h->smem, h->stream>>>(h->S, i, j, h->T); break;
+  }
+}
+
+template <int TR> static void launch_hlll_tr(const b200hh *h, const HlllArgs &A)
+{
+  const HBatch &S = h->S;
+  const int need  = (S.n + 31) / 32 + 1;
+  if (need <= 4)
+    hk_hlll<4, TR><<<hgrid(h), HW * 32, h->smem, h->stream>>>(S, A, h->T);
+  else if (need <= 8)
+    hk_hlll<8, TR><<<hgrid(h), HW * 32, h->smem, h->stream>>>(S, A, h->T);
+  else if (need <= 14)
+    hk_hlll<14, TR><<<hgrid(h), HW * 32, h->smem, h->stream>>>(S, A, h->T);
+  else
+    hk_hlll<32, TR><<<hgrid(h), HW * 32, h->smem, h->stream>>>(S, A, h->T);
+}
+
 static void launch_update_R_h(b200hh *h, int i, int last_j)
 {
   const HBatch &S = h->S;
@@ -1135,6 +1261,11 @@ int b200hh_create(b200hh_t **out, int batch, int d, int n, int flags, int device
 {
   if (!out || batch <= 0 || d <= 0 || n <= 0)
     return B200HH_EINVAL;
+  if ((flags & B200HH_INV_TRANSFORM) && !(flags & B200HH_TRANSFORM))
+  {
+    g_err = "b200hh_create: B200HH_INV_TRANSFORM needs B200HH_TRANSFORM (the reference updates u_inv_t only with u)";
+    return B200HH_EINVAL;
+  }
   int nd = 0;
   if (cudaGetDeviceCount(&nd) != cudaSuccess || nd <= device)
   {
@@ -1165,6 +1296,12 @@ int b200hh_create(b200hh_t **out, int batch, int d, int n, int flags, int device
   S.hist = nullptr;
   if (!rc && keep_history)
     rc |= hh_alloc(h, &S.hist, batch * dn * n);
+  const size_t dd = (size_t)batch * d * d;
+  h->tr           = (flags & B200HH_INV_TRANSFORM) ? HT_UINV : (flags & B200HH_TRANSFORM) ? HT_U : HT_NONE;
+  if (!rc && h->tr >= HT_U)
+    rc |= hh_alloc(h, &h->T.u, dd);
+  if (!rc && h->tr == HT_UINV)
+    rc |= hh_alloc(h, &h->T.uinvt, dd);
   if (rc)
   {
     for (void *p : h->allocs)
@@ -1176,17 +1313,29 @@ int b200hh_create(b200hh_t **out, int batch, int d, int n, int flags, int device
   h->smem = (size_t)HW * 2 * ((n + 1) & ~1) * sizeof(double);
   const void *fns[] = {(const void *)hk_init,        (const void *)hk_refresh_R_bf, (const void *)hk_refresh_R,
                        (const void *)hk_update_R<4>, (const void *)hk_update_R<8>, (const void *)hk_update_R<14>,
-                       (const void *)hk_update_R<32>, (const void *)hk_update_R_last, (const void *)hk_size_reduce,
+                       (const void *)hk_update_R<32>, (const void *)hk_update_R_last,
                        (const void *)hk_update_R_x32, (const void *)hk_update_R_last_cond,
-                       (const void *)hk_swap,        (const void *)hk_recover_R,   (const void *)hk_hlll<4>,
-                       (const void *)hk_hlll<8>,     (const void *)hk_hlll<14>,     (const void *)hk_hlll<32>};
+                       (const void *)hk_recover_R};
   for (const void *f : fns)
     CKH(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));  // process-wide: opt-in maximum, never lowered
+  switch (h->tr)
+  {
+  case HT_NONE: CKH(hh_kernel_attrs<HT_NONE>()); break;
+  case HT_U: CKH(hh_kernel_attrs<HT_U>()); break;
+  default: CKH(hh_kernel_attrs<HT_UINV>()); break;
+  }
   CKH(cudaMemsetAsync(S.b, 0, (size_t)batch * d * S.ldb * 8, h->stream));
   CKH(cudaMemsetAsync(S.bf, 0, batch * dn * 8, h->stream));
   CKH(cudaMemsetAsync(S.R, 0, batch * dn * 8, h->stream));
   CKH(cudaMemsetAsync(S.V, 0, batch * dn * 8, h->stream));
   CKH(cudaMemsetAsync(S.meta, 0, (size_t)batch * HM_STRIDE * 4, h->stream));
+  for (int64_t *m : {h->T.u, h->T.uinvt})
+    if (m)
+    {
+      CKH(cudaMemsetAsync(m, 0, dd * 8, h->stream));
+      hk_identity<<<batch, 128, 0, h->stream>>>(m, d);
+      CKH(cudaGetLastError());
+    }
   CKH(cudaStreamSynchronize(h->stream));
   *out = h;
   return 0;
@@ -1274,7 +1423,7 @@ int b200hh_update_R_last(b200hh_t *h, int i)
 }
 int b200hh_swap(b200hh_t *h, int i, int j)
 {
-  HH_CALL(i >= 0 && i < j && j < h->S.d, (hk_swap<<<hgrid(h), HW * 32, h->smem, h->stream>>>(h->S, i, j)))
+  HH_CALL(i >= 0 && i < j && j < h->S.d, launch_swap(h, i, j))
 }
 int b200hh_recover_R(b200hh_t *h, int i)
 {
@@ -1290,7 +1439,7 @@ int b200hh_size_reduce(b200hh_t *h, int k, int e, int st, int *reduced)
   if (!h || k <= 0 || k >= h->S.d || e > k || st < 0 || st > e)
     return B200HH_EINVAL;
   CKH(cudaSetDevice(h->device));
-  hk_size_reduce<<<hgrid(h), HW * 32, h->smem, h->stream>>>(h->S, k, e, st, h->d_red);
+  launch_size_reduce(h, k, e, st);
   if (reduced)
   {
     CKH(cudaMemcpyAsync(reduced, h->d_red, sizeof(int) * h->S.B, cudaMemcpyDeviceToHost, h->stream));
@@ -1299,6 +1448,41 @@ int b200hh_size_reduce(b200hh_t *h, int k, int e, int st, int *reduced)
   CKH(cudaGetLastError());
   return 0;
 }
+
+// U / U^-T (batch x d x d, dense on both sides) to or from the host; a NULL pointer skips that matrix, a non-NULL one for
+// a matrix the handle does not keep is refused before anything is copied
+static int copy_transform(b200hh_t *h, int64_t *u, int64_t *uinvt, bool to_device)
+{
+  if (!h)
+    return B200HH_EINVAL;
+  if ((u && !h->T.u) || (uinvt && !h->T.uinvt))
+  {
+    g_err = u && !h->T.u ? "b200hh_set/get_transform: the handle was created without B200HH_TRANSFORM"
+                         : "b200hh_set/get_transform: the handle was created without B200HH_INV_TRANSFORM";
+    return B200HH_EINVAL;
+  }
+  CKH(cudaSetDevice(h->device));
+  const size_t bytes = (size_t)h->S.B * h->S.d * h->S.d * sizeof(int64_t);
+  const std::pair<int64_t *, int64_t *> mats[] = {{u, h->T.u}, {uinvt, h->T.uinvt}};
+  for (const auto &m : mats)
+    if (m.first)
+    {
+      if (to_device)
+        CKH(cudaMemcpyAsync(m.second, m.first, bytes, cudaMemcpyHostToDevice, h->stream));
+      else
+        CKH(cudaMemcpyAsync(m.first, m.second, bytes, cudaMemcpyDeviceToHost, h->stream));
+    }
+  CKH(cudaStreamSynchronize(h->stream));
+  CKH(cudaGetLastError());
+  return 0;
+}
+
+int b200hh_set_transform(b200hh_t *h, const int64_t *u, const int64_t *u_inv_t)
+{
+  return copy_transform(h, (int64_t *)u, (int64_t *)u_inv_t, true);
+}
+
+int b200hh_get_transform(b200hh_t *h, int64_t *u, int64_t *u_inv_t) { return copy_transform(h, u, u_inv_t, false); }
 
 int b200hh_get_state(b200hh_t *h, double *R, double *V, double *bf, double *sigma, double *norm_square_b,
                      int64_t *row_expo, int64_t *expo_norm_square_b, int *meta)
@@ -1406,15 +1590,12 @@ int b200hh_hlll(b200hh_t *h, double delta, double eta, double theta, double c, i
   A.dR = h->d_hlll, A.eR = h->d_hlll + bd, A.prevR = h->d_hlll + 2 * bd;
   A.prevE = h->d_hlll_i, A.status = h->d_hlll_i + bd, A.iters = h->d_hlll_it;
   A.max_iter = 1000000ull + 64ull * S.d * S.d;
-  const int need = (S.n + 31) / 32 + 1;
-  if (need <= 4)
-    hk_hlll<4><<<hgrid(h), HW * 32, h->smem, h->stream>>>(S, A);
-  else if (need <= 8)
-    hk_hlll<8><<<hgrid(h), HW * 32, h->smem, h->stream>>>(S, A);
-  else if (need <= 14)
-    hk_hlll<14><<<hgrid(h), HW * 32, h->smem, h->stream>>>(S, A);
-  else
-    hk_hlll<32><<<hgrid(h), HW * 32, h->smem, h->stream>>>(S, A);
+  switch (h->tr)
+  {
+  case HT_NONE: launch_hlll_tr<HT_NONE>(h, A); break;
+  case HT_U: launch_hlll_tr<HT_U>(h, A); break;
+  default: launch_hlll_tr<HT_UINV>(h, A); break;
+  }
   CKH(cudaMemcpyAsync(status, A.status, (size_t)S.B * 4, cudaMemcpyDeviceToHost, h->stream));
   if (iterations)
     CKH(cudaMemcpyAsync(iterations, A.iters, (size_t)S.B * 8, cudaMemcpyDeviceToHost, h->stream));

@@ -6,6 +6,8 @@ import numpy as np
 from ._lib import B200Error, load
 
 HOUSEHOLDER_DEFAULT, HOUSEHOLDER_ROW_EXPO, HOUSEHOLDER_OP_FORCE_LONG = 0, 1, 4  # householder.h:26-32
+# include/b200hh.h (not reference values): the handle keeps U / also U^-T
+HOUSEHOLDER_TRANSFORM, HOUSEHOLDER_INV_TRANSFORM = 512, 1024
 _P = C.POINTER
 _done = False
 
@@ -21,6 +23,8 @@ def _lib():
         L.b200hh_destroy.restype = None
         L.b200hh_set_basis.argtypes = [vp, _P(C.c_int64)]
         L.b200hh_get_basis.argtypes = [vp, _P(C.c_int64)]
+        L.b200hh_set_transform.argtypes = [vp, _P(C.c_int64), _P(C.c_int64)]
+        L.b200hh_get_transform.argtypes = [vp, _P(C.c_int64), _P(C.c_int64)]
         for f in ("refresh_R_bf", "refresh_R", "update_R_last", "recover_R"):
             getattr(L, "b200hh_" + f).argtypes = [vp, i]
         L.b200hh_update_R.argtypes = [vp, i, i]
@@ -41,17 +45,33 @@ def _ck(rc, what):
 
 
 class MatHouseholder:
-    """MatHouseholder(b, flags): b (d, n) or (batch, d, n) int64; reference method names (householder.h)."""
+    """MatHouseholder(b, flags, device, keep_history, u, u_inv_t): b (d, n) or (batch, d, n) int64; reference method
+    names (householder.h).  u ((d, d) or (batch, d, d) int64) makes it the reference's MatHouseholder(b, u, u_inv_t,
+    flags) with a non-empty u: U starts as u and takes every integer row operation applied to b (.u reads it back);
+    u_inv_t likewise keeps U^-T (.u_inv_t) and needs u.  HOUSEHOLDER_TRANSFORM / HOUSEHOLDER_INV_TRANSFORM in flags
+    without the arrays start them at the identity."""
 
-    def __init__(self, b, flags=HOUSEHOLDER_ROW_EXPO | HOUSEHOLDER_OP_FORCE_LONG, device=0, keep_history=True):
+    def __init__(self, b, flags=HOUSEHOLDER_ROW_EXPO | HOUSEHOLDER_OP_FORCE_LONG, device=0, keep_history=True, u=None,
+                 u_inv_t=None):
         b = np.ascontiguousarray(b, dtype=np.int64)
         if b.ndim == 2:
             b = b[None]
         self.batch, self.d, self.n = b.shape
+        if u_inv_t is not None and u is None:
+            raise ValueError("u_inv_t needs u (the reference updates u_inv_t only when u is enabled)")
+        if u is not None:
+            flags |= HOUSEHOLDER_TRANSFORM
+        if u_inv_t is not None:
+            flags |= HOUSEHOLDER_INV_TRANSFORM
+        self.flags = flags
+        self.enable_transform = bool(flags & HOUSEHOLDER_TRANSFORM)
+        self.enable_inverse_transform = bool(flags & HOUSEHOLDER_INV_TRANSFORM)
         self._h = C.c_void_p()
         _ck(_lib().b200hh_create(C.byref(self._h), self.batch, self.d, self.n, flags, device, 1 if keep_history else 0),
             "b200hh_create")
         _ck(_lib().b200hh_set_basis(self._h, b.ctypes.data_as(_P(C.c_int64))), "set_basis")
+        if u is not None:
+            self.set_transform(u, u_inv_t)
 
     def close(self):
         if getattr(self, "_h", None) and self._h.value:
@@ -114,6 +134,41 @@ class MatHouseholder:
         _ck(_lib().b200hh_get_basis(self._h, b.ctypes.data_as(_P(C.c_int64))), "get_basis")
         return b
 
+    def _mats(self, a):
+        """(d, d) broadcast to every lattice, or (batch, d, d); None stays None"""
+        if a is None:
+            return None
+        a = np.asarray(a, np.int64)
+        if a.shape not in ((self.d, self.d), (self.batch, self.d, self.d)):
+            raise ValueError("expected shape (%d, %d) or (%d, %d, %d), got %s"
+                             % (self.d, self.d, self.batch, self.d, self.d, a.shape))
+        return np.ascontiguousarray(np.broadcast_to(a, (self.batch, self.d, self.d)))
+
+    def set_transform(self, u=None, u_inv_t=None):
+        """replaces U and / or U^-T: (d, d) (every lattice) or (batch, d, d) int64; None leaves that matrix alone"""
+        u, ut = self._mats(u), self._mats(u_inv_t)
+        p = lambda a: None if a is None else a.ctypes.data_as(_P(C.c_int64))
+        _ck(_lib().b200hh_set_transform(self._h, p(u), p(ut)), "set_transform")
+
+    def _get(self, inverse):
+        out = np.empty((self.batch, self.d, self.d), np.int64)
+        p = out.ctypes.data_as(_P(C.c_int64))
+        _ck(_lib().b200hh_get_transform(self._h, None if inverse else p, p if inverse else None), "get_transform")
+        return out
+
+    @property
+    def u(self):
+        """U of a transform object, (batch, d, d) int64"""
+        return self._get(False)
+
+    @property
+    def u_inv_t(self):
+        """U^-T of an inverse-transform object, (batch, d, d) int64"""
+        return self._get(True)
+
+    def sync(self):
+        _ck(_lib().b200hh_sync(self._h), "sync")
+
     def time_update_R(self, i, reps):
         ms = C.c_float()
         _ck(_lib().b200hh_time_update_R(self._h, i, reps, C.byref(ms)), "time_update_R")
@@ -123,16 +178,33 @@ class MatHouseholder:
 RED_HLLL_FAILURE, RED_HLLL_NORM_FAILURE, RED_HLLL_SR_FAILURE = 9, 10, 11  # defs.h:164-166
 
 
-def hlll_reduction(b, delta=0.99, eta=0.51, theta=0.001, c=0.1, device=0):
-    """hlll_reduction(ZZ_mat<long>& b, delta, eta, theta, c, HM_FAST, FT_DOUBLE) — fplll/wrapper.cpp:789-806 with
-    defaults LLL_DEF_DELTA / LLL_DEF_ETA / HLLL_DEF_THETA / HLLL_DEF_C (defs.h:143-151).  b: (d, n) or (batch, d, n)
-    int64.  Returns (reduced basis, status) — per lattice for a batch; the input array is not modified."""
+def hlll_reduction(b, delta=0.99, eta=0.51, theta=0.001, c=0.1, device=0, u=None, u_inv=None):
+    """hlll_reduction(ZZ_mat<long>& b, [u, [u_inv,]] delta, eta, theta, c, HM_FAST, FT_DOUBLE) — fplll/wrapper.cpp:789-806
+    and :1055-1087 with defaults LLL_DEF_DELTA / LLL_DEF_ETA / HLLL_DEF_THETA / HLLL_DEF_C (defs.h:143-151).  b: (d, n)
+    or (batch, d, n) int64.  Returns (reduced basis, status) — per lattice for a batch; the input array is not
+    modified.  u and u_inv (int64 arrays of b's leading shape with (d, d) last) are overwritten IN PLACE with the
+    transform of the call, starting from the identity as the reference does (gen_identity): u * b_in == b_out, and
+    u_inv = U^-1 (the reference runs with u_inv transposed and transposes it back).  u_inv needs u."""
     a = np.ascontiguousarray(b, dtype=np.int64)
     single = a.ndim == 2
-    m = MatHouseholder(a, HOUSEHOLDER_ROW_EXPO | HOUSEHOLDER_OP_FORCE_LONG, device=device, keep_history=True)
+    if u_inv is not None and u is None:
+        raise ValueError("u_inv needs u (the reference updates u_inv only when u is enabled)")
+    for name, t in (("u", u), ("u_inv", u_inv)):
+        if t is not None and (not isinstance(t, np.ndarray) or t.dtype != np.int64 or
+                              t.shape != a.shape[:-2] + (a.shape[-2], a.shape[-2])):
+            raise ValueError("%s must be an int64 array of shape %s" % (name, a.shape[:-2] + (a.shape[-2],) * 2))
+    eye = np.eye(a.shape[-2], dtype=np.int64)
+    m = MatHouseholder(a, HOUSEHOLDER_ROW_EXPO | HOUSEHOLDER_OP_FORCE_LONG, device=device, keep_history=True,
+                       u=None if u is None else eye, u_inv_t=None if u_inv is None else eye)
     try:
         st, _ = m.hlll(delta, eta, theta, c)
         out = m.get_basis()
+        uo = m.u if u is not None else None
+        ui = m.u_inv_t.transpose(0, 2, 1) if u_inv is not None else None
     finally:
         m.close()
+    if u is not None:
+        u[...] = uo[0] if single else uo
+    if u_inv is not None:
+        u_inv[...] = ui[0] if single else ui
     return (out[0], int(st[0])) if single else (out, st)

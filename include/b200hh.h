@@ -22,6 +22,19 @@ typedef struct b200hh b200hh_t;
 #define B200HH_DEFAULT 0
 #define B200HH_ROW_EXPO 1
 #define B200HH_OP_FORCE_LONG 4
+/* Not a reference value.  The handle also keeps the transform U of MatHouseholder(b, u, u_inv_t, flags) with a
+ * non-empty u (householder.h:41-135, enable_transform): int64, d x d per lattice, starting as the identity.  Both
+ * integer row operations of HLLL are applied to U with the same index: size_reduce's row_addmul_we(k, i, x, expo_add)
+ * adds lx * 2^expo * U[i] to U[k] with the lx and expo it uses for b (householder.cpp:455-559) and the same wrapping
+ * int64 arithmetic as Z_NR<long> (a shift by 64 or more gives 0, as on b), over all d columns of U (the reference's
+ * u[i].addmul_si(u[j], x) has no n_known_cols bound); swap(i, j) swaps rows i and j of U (householder.cpp:372-398).
+ * HLLL never negates a row, so U equals the reference's bit for bit.  No decision reads U: a transform handle ends every
+ * call with the same b, R, V, sigma, bf, status and iteration count as a handle without it. */
+#define B200HH_TRANSFORM 512
+/* Not a reference value.  With B200HH_TRANSFORM only (B200HH_EINVAL otherwise: the reference updates u_inv_t only when
+ * u is enabled): the handle also keeps U^-T, the reference's u_inv_t, starting as the identity.  row_addmul_we(k, i, ...)
+ * adds (-lx) * 2^expo * U^-T[k] to U^-T[i]; swap(i, j) swaps its rows i and j.  U * (U^-T)^T = I holds mod 2^64. */
+#define B200HH_INV_TRANSFORM 1024
 
 #define B200HH_EINVAL (-1)
 #define B200HH_ENODEV (-2)
@@ -42,6 +55,13 @@ int b200hh_create(b200hh_t **out, int batch, int d, int n, int flags, int device
 void b200hh_destroy(b200hh_t *h);
 int b200hh_set_basis(b200hh_t *h, const int64_t *b);
 int b200hh_get_basis(b200hh_t *h, int64_t *b);
+
+/* Replace / read back U and U^-T: batch*d*d int64 each, row-major, lattice-major.  Either pointer may be NULL (that matrix
+ * is left alone); a non-NULL pointer for a matrix the handle does not keep (no B200HH_TRANSFORM, no
+ * B200HH_INV_TRANSFORM) gives B200HH_EINVAL and nothing is copied.  set_basis and hlll leave U and U^-T where they are:
+ * hlll continues from the current U. */
+int b200hh_set_transform(b200hh_t *h, const int64_t *u, const int64_t *u_inv_t);
+int b200hh_get_transform(b200hh_t *h, int64_t *u, int64_t *u_inv_t);
 
 /* refresh_R_bf(i) householder.cpp:186-245; refresh_R(i) :247-261 */
 int b200hh_refresh_R_bf(b200hh_t *h, int i);
@@ -73,7 +93,8 @@ int b200hh_time_update_R(b200hh_t *h, int i, int reps, float *ms_update_mean);
  * the batch; the handle must have been created with keep_history (recover_R reads R_history).
  * status[batch]: RedStatus per lattice (0 RED_SUCCESS, 10 RED_HLLL_NORM_FAILURE, 11 RED_HLLL_SR_FAILURE; 9 if the
  * device-side iteration guard trips — the reference has no such guard).  iterations[batch] (optional): main-loop
- * trips.  The reduced bases are read back with b200hh_get_basis. */
+ * trips.  The reduced bases are read back with b200hh_get_basis; on a B200HH_TRANSFORM handle U (and U^-T) have taken
+ * every row operation of the call, starting from what they held (b200hh_get_transform). */
 int b200hh_hlll(b200hh_t *h, double delta, double eta, double theta, double c, int *status, uint64_t *iterations);
 int b200hh_sync(b200hh_t *h);
 
