@@ -5,6 +5,7 @@
 #include "../../include/b200bkz.h"
 #include "../../include/b200enum.h"
 #include "../../include/b200gso.h"
+#include <algorithm>
 #include <chrono>
 #include <cmath>
 #include <cstdio>
@@ -77,7 +78,7 @@ class Driver
 {
 public:
   Driver(b200bkz *ctx, b200gso_t *g, int d, const b200bkz_param &top, b200bkz_stats *st)
-      : ctx(ctx), g(g), d(d), top(top), st(st), rng(top.seed ? top.seed : 0x9e3779b97f4a7c15ull)
+      : ctx(ctx), g(g), num_rows(d), top(top), st(st), rng(top.seed ? top.seed : 0x9e3779b97f4a7c15ull)
   {
     lll_delta = top.delta < 1 ? top.delta : 0.99;  // bkz.cpp:862
     // the fixed region unless the caller asks for the shrinking radius (only pruned calls: without pruning the shrinking
@@ -256,7 +257,7 @@ public:
     const std::vector<int> preproc = strategy(block_size).preproc;
     for (int pb : preproc)
     {
-      int dummy_kappa_max = d;
+      int dummy_kappa_max = num_rows;
       b200bkz_param prepar;
       b200bkz_default_param(&prepar, pb);
       prepar.flags = B200BKZ_GH_BND;
@@ -377,6 +378,13 @@ public:
         st->sec_get += now_s() - tg;
         st->get_calls++;
       }
+      // a zero r(i, i) (a dependent row inside the reduced range) has no place in the enumerator: its normalisation and
+      // radius would be meaningless and the walk need not end
+      for (int i = 0; i < block_size; i++)
+        if (!(rmant[i] > 0))
+          throw std::runtime_error("BKZ block [" + std::to_string(kappa) + ", " + std::to_string(kappa + block_size) +
+                                   ") has r(" + std::to_string(kappa + i) + ", " + std::to_string(kappa + i) +
+                                   ") = 0: the rows are linearly dependent");
       long max_dist_expo = rexpo[first - kappa];
       double max_dist    = rmant[first - kappa];
       if (dual)
@@ -507,7 +515,7 @@ public:
   // sd_tour, bkz.cpp:443-463: a dual tour backwards, then a truncated primal tour forwards
   bool sd_tour(const b200bkz_param &par, int min_row, int max_row)
   {
-    int dummy_kappa_max = d;
+    int dummy_kappa_max = num_rows;
     bool clean          = true;
     clean &= trunc_dtour(par, min_row, max_row);
     clean &= trunc_tour(dummy_kappa_max, par, min_row, max_row);
@@ -607,10 +615,10 @@ public:
     {
       int ok = 1;
       GCK(b200gso_update_gso(g, &ok));
-      sld_potential = slide_potential(0, d, top.block_size);
+      sld_potential = slide_potential(0, num_rows, top.block_size);
     }
     if (sd)  // sd-bkz starts with a dual tour, whose size reductions need LLL-reduced lower blocks (bkz.cpp:573-577; the
-      lll(0, 0, d, nullptr, false);  // reference ignores this call's status)
+      lll(0, 0, num_rows, nullptr, false);  // reference ignores this call's status)
     int no_dec           = -1;
     double old_slope     = std::numeric_limits<double>::max();
     int kappa_max        = -1;
@@ -631,7 +639,7 @@ public:
       if (flags & B200BKZ_AUTO_ABORT)
       {
         // BKZAutoAbort::test_abort, bkz.cpp:800-809
-        const double new_slope = -current_slope(0, d);
+        const double new_slope = -current_slope(0, num_rows);
         if (no_dec == -1 || new_slope < top.auto_abort_scale * old_slope)
           no_dec = 0;
         else
@@ -641,11 +649,11 @@ public:
           break;
       }
       if (sd)
-        clean = sd_tour(top, 0, d);
+        clean = sd_tour(top, 0, num_rows);
       else if (sld)
-        clean = slide_tour(top, 0, d);
+        clean = slide_tour(top, 0, num_rows);
       else
-        clean = tour(i, kappa_max, top, 0, d);
+        clean = tour(i, kappa_max, top, 0, num_rows);
       st->tours = i + 1;
       if (flags & B200BKZ_VERBOSE)
       {
@@ -655,39 +663,77 @@ public:
         fprintf(stderr, "End of %s loop %d, time = %.3fs, r_0 = %.6g, enum nodes = 2^%.2f\n", algorithm, i,
                 now_s() - t_start, ldexp(m, (int)e), log2((double)st->enum_nodes + 1));
       }
-      if (clean || top.block_size >= d)
+      if (clean || top.block_size >= num_rows)
         break;
     }
-    int dummy_kappa_max = d;
+    int dummy_kappa_max = num_rows;
     if (sd)  // hkz-reduce the last window, which SD-BKZ leaves unreduced (bkz.cpp:626-641)
-      hkz(dummy_kappa_max, top, std::max(d - top.block_size, 0), d);
+      hkz(dummy_kappa_max, top, std::max(num_rows - top.block_size, 0), num_rows);
     if (sld)
     {
       // hkz-reduce the blocks, which slide reduction leaves only SVP- and dual-SVP-reduced (bkz.cpp:642-665)
-      int p = d / top.block_size;
-      if (d % top.block_size)
+      int p = num_rows / top.block_size;
+      if (num_rows % top.block_size)
         ++p;
       for (int j = 0; j < p; ++j)
       {
         const int kappa = j * top.block_size + 1;
-        hkz(dummy_kappa_max, top, kappa, std::min(d, kappa + top.block_size - 1));
+        hkz(dummy_kappa_max, top, kappa, std::min(num_rows, kappa + top.block_size - 1));
       }
     }
     return final_status;
   }
 
   double delta() const { return top.delta; }
+  // BKZReduction's constructor, bkz.cpp:35: the rows the tours reduce end before the trailing zero rows
+  void set_num_rows(int rows) { num_rows = rows; }
 
 private:
   b200bkz *ctx;
   b200gso_t *g;
-  int d;
+  int num_rows;  // rows 0..num_rows-1: the basis without its trailing zero rows (bkz.cpp:35)
   const b200bkz_param &top;
   b200bkz_stats *st;
   std::mt19937_64 rng;
   double lll_delta;
   Strategy tmp;
 };
+
+// zeros_last / zeros_first (util.cpp:257-287) on the host arrays: rotate the rows so that row mid comes first, in b
+// (d x n) and, when given, u (d x d)
+void rotate_rows(int64_t *b, int d, int n, int64_t *u, int mid)
+{
+  if (mid <= 0 || mid >= d)
+    return;
+  std::rotate(b, b + (size_t)mid * n, b + (size_t)d * n);
+  if (u)
+    std::rotate(u, u + (size_t)mid * d, u + (size_t)d * d);
+}
+bool row_is_zero(const int64_t *b, int n, int i)
+{
+  for (int j = 0; j < n; j++)
+    if (b[(size_t)i * n + j] != 0)
+      return false;
+  return true;
+}
+// the leading zero rows to the end (bkz.cpp:869-870 under BKZ_NO_LLL)
+void zeros_last(int64_t *b, int d, int n, int64_t *u)
+{
+  int i = 0;
+  while (i < d && row_is_zero(b, n, i))
+    i++;
+  rotate_rows(b, d, n, u, i);
+}
+// the number of rows before the trailing zero rows (BKZReduction::num_rows, bkz.cpp:35)
+int nonzero_prefix(const int64_t *b, int d, int n)
+{
+  int i = d;
+  while (i > 0 && row_is_zero(b, n, i - 1))
+    i--;
+  return i;
+}
+// the trailing zero rows to the front (bkz.cpp:925)
+void zeros_first(int64_t *b, int d, int n, int64_t *u) { rotate_rows(b, d, n, u, nonzero_prefix(b, d, n)); }
 
 }  // namespace
 
@@ -786,6 +832,8 @@ static int bkz_reduce(b200bkz_t *h, int d, int n, int64_t *b, int64_t *u, const 
   if (!stats)
     stats = &local;
   memset(stats, 0, sizeof(*stats));
+  if (param->flags & B200BKZ_NO_LLL)
+    zeros_last(b, d, n, u);  // bkz.cpp:869-870; with the wrapper LLL, LLL itself moves zero rows to the end
   b200gso_t *g = nullptr;
   int rc       = b200gso_create(&g, 1, d, n, B200GSO_ROW_EXPO | (u ? B200GSO_TRANSFORM : 0), h->devs[0]);  // bkz.cpp:819-820
   if (rc)
@@ -801,7 +849,9 @@ static int bkz_reduce(b200bkz_t *h, int d, int n, int64_t *b, int64_t *u, const 
     if (u)
       GCK(b200gso_set_transform(g, u));  // the caller's U (bkz.cpp:857-859 starts it at the identity)
     Driver drv(h, g, d, *param, stats);
-    double tb = now_s();
+    double tb         = now_s();
+    int num_rows      = d;
+    bool wrapper_fail = false;
     try
     {
       if (!(param->flags & B200BKZ_NO_LLL))
@@ -809,15 +859,25 @@ static int bkz_reduce(b200bkz_t *h, int d, int n, int64_t *b, int64_t *u, const 
         // the reference runs its wrapper LLL here (bkz.cpp:869-876); in the int64 regime that is LLL(delta, 0.51).
         // A failure of this LLL (RED_BABAI_FAILURE on an fp64-fragile basis) is the call's status, not an exception.
         long swaps;
+        wrapper_fail = true;
         drv.lll(0, 0, d, &swaps);
+        wrapper_fail = false;
       }
       else
       {
         int ok = 1;
         GCK(b200gso_update_gso(g, &ok));
       }
-      stats->slope_before = drv.current_slope(0, d);
       {
+        // the tours reduce the rows before the trailing zero rows only (bkz.cpp:35): no block ever holds a zero row
+        std::vector<int64_t> cur((size_t)d * n);
+        GCK(b200gso_get_basis(g, cur.data()));
+        num_rows = nonzero_prefix(cur.data(), d, n);
+        drv.set_num_rows(num_rows);
+      }
+      if (num_rows > 0)
+      {
+        stats->slope_before = drv.current_slope(0, num_rows);
         double m;
         long e;
         drv.r_exp(0, m, e);
@@ -825,7 +885,7 @@ static int bkz_reduce(b200bkz_t *h, int d, int n, int64_t *b, int64_t *u, const 
       }
       stats->sec_lll = 0, stats->lll_calls = 0;
       tb            = now_s();
-      stats->status = drv.bkz();
+      stats->status = num_rows > 0 ? drv.bkz() : 0;  // a zero basis has nothing to reduce
     }
     catch (RedFailure &f)
     {
@@ -857,9 +917,10 @@ static int bkz_reduce(b200bkz_t *h, int d, int n, int64_t *b, int64_t *u, const 
     }
 #endif
     stats->sec_other = stats->sec_total - stats->sec_enum - stats->sec_lll;
-    if (stats->status == 0 || stats->status == B200_RED_BKZ_LOOPS_LIMIT || stats->status == B200_RED_BKZ_TIME_LIMIT)
+    if (num_rows > 0 &&
+        (stats->status == 0 || stats->status == B200_RED_BKZ_LOOPS_LIMIT || stats->status == B200_RED_BKZ_TIME_LIMIT))
     {
-      stats->slope_after = drv.current_slope(0, d);
+      stats->slope_after = drv.current_slope(0, num_rows);
       double m;
       long e;
       drv.r_exp(0, m, e);
@@ -868,6 +929,8 @@ static int bkz_reduce(b200bkz_t *h, int d, int n, int64_t *b, int64_t *u, const 
     GCK(b200gso_get_basis(g, b));
     if (u)
       GCK(b200gso_get_transform(g, u));
+    if (!wrapper_fail)
+      zeros_first(b, d, n, u);  // bkz.cpp:925 (a failed wrapper LLL returns before it, bkz.cpp:874-875)
   }
   catch (std::exception &ex)
   {

@@ -86,7 +86,9 @@ void b200bkz_destroy(b200bkz_t *h);
  * Block sizes without a strategy use the reference's EmptyStrategy (no preprocessing, no pruning). */
 int b200bkz_add_strategy(b200bkz_t *h, int block_size, const int *preproc, int n_preproc, const double *gh_factor,
                          const double *expectation, const double *coefficients, int n_prune);
-/* bkz_reduction on a d x n int64 basis, in place.  Returns 0 or a negative error; RedStatus in stats->status. */
+/* bkz_reduction on a d x n int64 basis, in place.  Returns 0 or a negative error; RedStatus in stats->status.  As in
+ * the reference (bkz.cpp:35, 869-870, 925), zero rows are moved to the end first (by the preliminary LLL, or by
+ * zeros_last under BKZ_NO_LLL), the tours reduce only the rows before them, and they end up first. */
 int b200bkz_reduce(b200bkz_t *h, int d, int n, int64_t *b, const b200bkz_param *param, b200bkz_stats *stats);
 /* bkz_reduction(b, u, param) (bkz.h:357-426, BKZReduction with a transform, bkz.cpp:822-836): the same call, and u
  * (d x d int64, row-major, in/out) takes every integer row operation applied to b.  The caller initialises u as for
